@@ -1,4 +1,4 @@
-"""accelerated_features_b200: XFeat inference hot path as hand-written sm_100a CUDA kernels (drop-in `XFeat` class)."""
+"""accelerated_features_b200: XFeat inference hot path as hand-written sm_90a CUDA kernels (drop-in `XFeat` class)."""
 from .xfeat import XFeat  # noqa: F401
 
 __all__ = ["XFeat"]

@@ -1,11 +1,11 @@
-"""ctypes binding of libxfeat_sm100.so (include/xfeat_b200.h).  No CPU fallback: a missing library is an error."""
+"""ctypes binding of libxfeat_sm90.so (include/xfeat_b200.h).  No CPU fallback: a missing library is an error."""
 from __future__ import annotations
 
 import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libxfeat_sm100.so")
+LIB_PATH = os.path.join(_HERE, "libxfeat_sm90.so")
 _lib = None
 ABI_VERSION = 2      # XFEAT_ABI_VERSION of include/xfeat_b200.h
 N_OVERFLOW = -1      # XF_N_OVERFLOW

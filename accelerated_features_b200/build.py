@@ -1,4 +1,4 @@
-"""Build libxfeat_sm100.so in-tree with nvcc (sm_100a only).  `python -m accelerated_features_b200.build`"""
+"""Build libxfeat_sm90.so in-tree with nvcc (sm_90a only).  `python -m accelerated_features_b200.build`"""
 from __future__ import annotations
 
 import concurrent.futures as cf
@@ -10,10 +10,10 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.path.join(HERE, "libxfeat_sm100.so")
+LIB = os.path.join(HERE, "libxfeat_sm90.so")
 OBJ = os.path.join(HERE, "build")
 SOURCES = ["api.cu", "prep.cu", "stem.cu", "conv_simt.cu", "conv_tc.cu", "conv_tc_halo.cu", "head_chain_tc.cu", "heads.cu", "sparse.cu", "dense.cu", "mnn.cu", "mnn_tc.cu", "mnn_fast.cu", "refine.cu", "mlp_tc.cu", "helpers.cu", "ransac.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "--expt-relaxed-constexpr",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "-Xptxas", "-v"]
 
 
@@ -60,7 +60,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
     if verbose:
         for _, log in results:
             sys.stderr.write(log)
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout + r.stderr)

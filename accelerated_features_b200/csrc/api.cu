@@ -12,7 +12,7 @@ namespace xf {
 
 static thread_local char g_err[1024] = "";
 unsigned long long g_launches = 0;
-int g_conv_impl = 2;  // 0 = fp32 CUDA-core convs everywhere, 1 = tcgen05 for the 64->64 stride-1 layers (default)
+int g_conv_impl = 2;  // 0 = fp32 CUDA-core convs everywhere, 1 = wgmma for the tensor-core layers, 2 = 1 + halo-patch 3x3 (default)
 
 // (device, kernel) -> largest dynamic shared-memory size opted into so far
 int ensure_dyn_smem(const void* func, size_t bytes) {
@@ -81,8 +81,8 @@ extern "C" int xfeat_create(xfeat_ctx** out, int device, const float* packed_hos
   XF_REQUIRE(guard.ok, "create: cudaSetDevice(%d) failed", device);
   cudaDeviceProp prop;
   XF_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    xf::set_error("create: device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    xf::set_error("create: device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     return XF_E_UNSUPPORTED;
   }
   xfeat_ctx* c = new xfeat_ctx();
@@ -169,11 +169,11 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
     XF_RUN(launch_conv_layer(ctx, L_B4_2, ws.t16b, IN_NHWC, B, H16, W16, ws.x4, st));
     XF_RUN(launch_conv_layer(ctx, L_B5_0, ws.x4, IN_NHWC, B, H16, W16, ws.t32a, st));                // block5, model.py:143
   } else {
-    // ---- block2 .. block5.0 on tcgen05; activations between tensor-core layers travel as split fp16 [hi | lo] ----
+    // ---- block2 .. block5.0 on the tensor cores (wgmma); activations between tensor-core layers travel as split fp16 [hi | lo] ----
     __half *s4a = (__half*)ws.x1s, *s4b = (__half*)ws.t4a, *s4c = (__half*)ws.x2;
     __half *s8a = (__half*)ws.t8a, *s8b = (__half*)ws.t8b, *s16a = (__half*)ws.t16a, *s16b = (__half*)ws.t16b;
     if (g_conv_impl == 2) {
-      // block1.0/1.1 on CUDA cores (K = 9 / 36), block1.2 (halo) and block1.3 + skip1 (stride 2) on tcgen05 with 32-byte
+      // block1.0/1.1 on CUDA cores (K = 9 / 36), block1.2 (halo) and block1.3 + skip1 (stride 2) on the tensor cores with 32-byte
       // operand rows [hi(8)|lo(8)]                                                 model.py:43-48,139-140
       XF_RUN(launch_stem_chain(ctx->h_weights, ctx->table, d_xn, ws.a1, ws.a2, ws.a3, nullptr, nullptr, B, H, W, st, 1));
       XF_RUN(launch_conv_tc(ctx, L_B1_2, (const __half*)ws.a2, B, H / 2, W / 2, (__half*)ws.a3, nullptr, st));
@@ -223,7 +223,7 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
     XF_RUN(launch_conv_tc(ctx, L_FU_1, sf1, B, H8, W8, sf2, nullptr, st));
     XF_RUN(launch_conv_tc(ctx, L_FU_2, sf2, B, H8, W8, s8a, d_feats, st));      // fp32 feats for the samplers + split for the head
     if (g_conv_impl == 2) {
-      // fused head chains: activations stay in shared memory / TMEM between the 1x1 layers (head_chain_tc.cu)
+      // fused head chains: activations stay in shared memory / registers between the 1x1 layers (head_chain_tc.cu)
       XF_RUN(launch_head_chain(ctx, 1, s8a, B, H8, W8, d_reliability, nullptr, st));                 // model.py:151
       XF_RUN(launch_head_chain(ctx, 0, d_xn, B, H8, W8, d_heat, d_kpt_logits, st));   // unfold8 (model.py:152) inside; + xfeat.py:242-247
       return XF_OK;

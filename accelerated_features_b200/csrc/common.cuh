@@ -1,4 +1,4 @@
-// Shared helpers for libxfeat_sm100.so (sm_100a only).
+// Shared helpers for libxfeat_sm90.so (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -119,22 +119,11 @@ __device__ __forceinline__ float sparse_src_coord(int p, int size_pos, int size_
 }
 
 // ATen upsample_bilinear2d source index (align_corners=False): src = scale*(dst+0.5)-0.5 clamped at 0.
-// packed fp32 pairs (sm_100: FFMA2 / FMUL2): two independent IEEE round-to-nearest operations per instruction
+// fp32 pairs: two independent IEEE round-to-nearest operations
 __device__ __forceinline__ float2 f2_fma(float2 a, float2 b, float2 c) {
-  float2 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&r))
-      : "l"(*reinterpret_cast<const unsigned long long*>(&a)), "l"(*reinterpret_cast<const unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<const unsigned long long*>(&c)));
-  return r;
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 f2_mul(float2 a, float2 b) {
-  float2 r;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&r))
-      : "l"(*reinterpret_cast<const unsigned long long*>(&a)), "l"(*reinterpret_cast<const unsigned long long*>(&b)));
-  return r;
-}
+__device__ __forceinline__ float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 struct LinTap {
   int i0, i1;
@@ -175,7 +164,7 @@ namespace xf {
 enum { IN_NHWC = 0, IN_UNFOLD8 = 1 };
 int launch_conv_layer(const xfeat_ctx* ctx, int layer, const float* in, int in_mode, int B, int Hi, int Wi,
                       float* out, cudaStream_t st, const int* n_live = nullptr, __half* out_split = nullptr);
-extern int g_conv_impl;  // 0 = fp32 CUDA cores, 1 = tcgen05 (per-tap operand loads), 2 = tcgen05 + halo-patch reuse for 3x3/s1
+extern int g_conv_impl;  // 0 = fp32 CUDA cores, 1 = wgmma (per-tap operand loads), 2 = wgmma + halo-patch reuse for 3x3/s1
 bool conv_tc_eligible(int layer);
 int launch_conv_tc_halo(const xfeat_ctx* ctx, int layer, const __half* in_split, int B, int H, int W, __half* out_split,
                         float* out_f32, cudaStream_t st);

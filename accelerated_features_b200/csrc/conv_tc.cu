@@ -1,5 +1,5 @@
-// 64->64 convolutions (3x3 pad 1 / 1x1, stride 1) as implicit GEMM on the 5th-generation tensor cores:
-// TMA-fed shared-memory operands, tcgen05.mma with fp32 accumulators in TMEM, bias+ReLU epilogue from TMEM.
+// 64->64 convolutions (3x3 pad 1 / 1x1, stride 1) as implicit GEMM on the Hopper tensor cores:
+// TMA-fed shared-memory operands, wgmma with fp32 register accumulators, bias+ReLU epilogue.
 // Used for block3.1/3.2, block4.1/4.2, block_fusion.0-2, heatmap_head.0-1, keypoint_head.0-2 (model.py:55-92) -- 48 % of
 // the network's FLOPs.
 //
@@ -13,8 +13,9 @@
 //   * the A operand of tap (dy,dx) is the input patch shifted by (dy-1, dx-1): ONE 4-D TMA box {64 ch, TW, TH, 1} per
 //     term, 128B-swizzled K-major, out-of-image coordinates zero-filled by the TMA unit (= the conv's zero padding);
 //   * the folded, pre-split weights of all taps stay resident in shared memory for the life of the (persistent) CTA;
-//   * warp 0 = TMA producer, warp 1 = single-thread MMA issuer, warps 2-5 = epilogue (one TMEM lane quarter each);
-//     the accumulator is double buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
+//   * warps 0-3 = one warpgroup that issues the wgmmas (two 64-row slabs per tile) and runs the epilogue, one pixel row per
+//     thread (the accumulator fragments are handed over through a 16 KB staging buffer); warp 4 = TMA producer, which runs
+//     up to NS taps ahead, so the operand loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda_fp16.h>
 
 #include <vector>
@@ -24,8 +25,7 @@
 
 namespace xf {
 
-constexpr int CT_THREADS = 192;    // conv_tc128_kernel: warp 0 TMA, warp 1 MMA, warps 2-5 epilogue
-constexpr int CT_THREADS2 = 320;   // conv_tc_kernel: two epilogue groups (warps 2-5 / 6-9) alternate tiles
+constexpr int CT_THREADS = 160;    // warps 0-3: wgmma + epilogue warpgroup, warp 4: TMA producer
 constexpr int CT_ABOX = 128 * 128;   // bytes: 128 pixels x 128 B (64 halves)
 
 // CINP = padded input channels per term (64: two boxes per tap, hi and lo; 32: ONE box per tap whose 128-byte rows are
@@ -38,23 +38,20 @@ struct ConvTcCfg {
   static constexpr int ROWB = (CINP == 8) ? 32 : 128;                 // operand row bytes ([hi(8)|lo(8)] halves for the stem)
   static constexpr int KSTEPS = ROWB / 32;
   static constexpr int A_BOXES = (CINP == 64) ? 2 : 1;
-  // CINP = 8: a tap is only 4 KB and one UMMA, so a pipeline stage carries ALL taps of a tile (one barrier round trip per
+  // CINP = 8: a tap is only 4 KB and one K-step, so a pipeline stage carries ALL taps of a tile (one barrier round trip per
   // tile instead of per tap); otherwise one tap per stage.
   static constexpr int TPS = (CINP == 8) ? TAPS : 1;
   static constexpr int A_TAP = A_BOXES * 128 * ROWB;
   static constexpr int A_STAGE = TPS * A_TAP;
   static constexpr int W_GROUP = NOUT * ROWB;                         // bytes
   static constexpr size_t W_BYTES = (size_t)TAPS * 2 * W_GROUP;
-  static constexpr int NS_MAX = (int)((227 * 1024 - 2048 - W_BYTES) / A_STAGE);
+  static constexpr int NS_MAX = (int)((227 * 1024 - 2048 - W_BYTES - tc::STG_BYTES) / A_STAGE);
   static constexpr int NS_CAP = (CINP == 8) ? 4 : 6;
   static constexpr int NS = NS_MAX > NS_CAP ? NS_CAP : NS_MAX;        // A stages (one tap each)
   static constexpr size_t A_BYTES = (size_t)NS * A_STAGE;
-  static constexpr size_t SMEM = 1024 + W_BYTES + A_BYTES + 1536;
-  // accumulator per buffer: columns [0,NOUT) = terms against weight group 0, [NOUT,2*NOUT) = against group 1: a single UMMA
-  // with N = 2*NOUT reads the activation operand once for both groups (the layers are shared-memory-bandwidth bound).
-  static constexpr int ACC_COLS = 2 * NOUT;
-  static constexpr int NACC = (512 / ACC_COLS) > 8 ? 8 : (512 / ACC_COLS);   // accumulator ring (see conv_tc_halo.cu)
-  static constexpr int TMEM_COLS = NACC * ACC_COLS;
+  static constexpr size_t SMEM = 1024 + W_BYTES + A_BYTES + tc::STG_BYTES + 1536;
+  // accumulator: columns [0,NOUT) = terms against weight group 0, [NOUT,2*NOUT) = against group 1: a single wgmma with
+  // N = 2*NOUT reads the activation operand once for both groups (the layers are shared-memory-bandwidth bound).
   static_assert(NS >= 2, "need at least two A stages");
   static_assert(CINP == 8 || CINP == 32 || CINP == 64, "CINP");
   static_assert(NOUT == 32 || NOUT == 64, "NOUT");
@@ -81,21 +78,18 @@ struct ConvTcParams {
 };
 
 template <int KS, int CINP, int NOUT>
-__global__ void __launch_bounds__(CT_THREADS2, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams P) {
+__global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams P) {
   using C = ConvTcCfg<KS, CINP, NOUT>;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sW = base;
   unsigned char* sA = base + C::W_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + C::A_BYTES);
+  float* sStg = reinterpret_cast<float*>(base + C::W_BYTES + C::A_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + C::A_BYTES + tc::STG_BYTES);
   uint64_t* w_full = bars;
   uint64_t* a_full = bars + 1;                 // [NS]
   uint64_t* a_empty = bars + 1 + C::NS;        // [NS]
-  constexpr int NACC = C::NACC;
-  uint64_t* acc_full = bars + 1 + 2 * C::NS;   // [NACC]
-  uint64_t* acc_empty = acc_full + NACC;       // [NACC]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + NACC);
-  float* sBias = reinterpret_cast<float*>(tmem_slot + 2);
+  float* sBias = reinterpret_cast<float*>(bars + 1 + 2 * C::NS);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int TW = 1 << P.tw_log2, TH = 128 >> P.tw_log2;
@@ -109,30 +103,19 @@ __global__ void __launch_bounds__(CT_THREADS2, 1) conv_tc_kernel(const __grid_co
     const int c = threadIdx.x % NOUT, wb = threadIdx.x / NOUT;
     sSkip[threadIdx.x] = (P.skip_w != nullptr && c < 24) ? __ldg(P.skip_w + wb * 24 + c) : 0.f;
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
     tc::mbar_init(w_full, 1);
     for (int i = 0; i < C::NS; ++i) {
       tc::mbar_init(&a_full[i], 1);
-      tc::mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < NACC; ++i) {
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 4);
+      tc::mbar_init(&a_empty[i], 4);   // one arrival per consumer warp
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, C::TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (tc::elect_one()) {
       // ---------------- TMA producer ----------------
       tc::mbar_expect_tx(w_full, (uint32_t)C::W_BYTES);
@@ -159,78 +142,72 @@ __global__ void __launch_bounds__(CT_THREADS2, 1) conv_tc_kernel(const __grid_co
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      // ---------------- MMA issuer ----------------
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, NOUT);
-      constexpr uint32_t idesc2 = tc::make_idesc(/*F16*/ 0, 128, 2 * NOUT);
-      tc::mbar_wait(w_full, 0);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-        const int a = tcount % NACC;
-        tc::mbar_wait(&acc_empty[a], ((tcount / NACC) & 1) ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem + a * C::ACC_COLS;
-        for (int tap0 = 0; tap0 < C::TAPS; tap0 += C::TPS, ++it) {
-          const int s = it % C::NS;
-          tc::mbar_wait(&a_full[s], (it / C::NS) & 1);
-          tc::tc_fence_after();
+  } else {
+    // ---------------- wgmma + epilogue warpgroup: thread r owns pixel r of the tile ----------------
+    constexpr int N2 = 2 * NOUT;
+    constexpr uint32_t HALF = (64 * C::ROWB) >> 4;   // descriptor offset of rows 64-127
+    const int r = threadIdx.x;
+    const int ph_ = r >> P.tw_log2, pw_ = r & (TW - 1);
+    float acc0[NOUT], acc1[NOUT];                    // rows 0-63 / 64-127, N2 columns each
+    tc::mbar_wait(w_full, 0);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      for (int tap0 = 0; tap0 < C::TAPS; tap0 += C::TPS, ++it) {
+        const int s = it % C::NS;
+        tc::mbar_wait(&a_full[s], (it / C::NS) & 1);
+        tc::wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < C::TPS; ++j) {
-            const int tap = tap0 + j;
-            const uint32_t a_addr = tc::smem_u32(sA + (size_t)s * C::A_STAGE + (size_t)j * C::A_TAP);
-            const uint32_t w_addr = tc::smem_u32(sW + (size_t)tap * 2 * C::W_GROUP);
-            const uint64_t a0 = tc::make_desc_rows<C::ROWB>(a_addr);
-            const uint64_t w0 = tc::make_desc_rows<C::ROWB>(w_addr);   // group 0, and (N = 2*NOUT) groups [0 ; 1] stacked
-            if (C::A_BOXES == 2) {
-              const uint64_t a1 = tc::make_desc_sw128(a_addr + CT_ABOX, 1024);
+        for (int j = 0; j < C::TPS; ++j) {
+          const int tap = tap0 + j;
+          const uint32_t a_addr = tc::smem_u32(sA + (size_t)s * C::A_STAGE + (size_t)j * C::A_TAP);
+          const uint32_t w_addr = tc::smem_u32(sW + (size_t)tap * 2 * C::W_GROUP);
+          const uint64_t a0 = tc::make_desc_rows<C::ROWB>(a_addr);
+          const uint64_t w0 = tc::make_desc_rows<C::ROWB>(w_addr);   // group 0, and (N = 2*NOUT) groups [0 ; 1] stacked
+          if (C::A_BOXES == 2) {
+            const uint64_t a1 = tc::make_desc_sw128(a_addr + CT_ABOX, 1024);
 #pragma unroll
-              for (int k = 0; k < 4; ++k) tc::umma_f16(d, a0 + 2 * k, w0 + 2 * k, idesc2, (tap | k) ? 1u : 0u);  // hi.whi | hi.wlo
+            for (int k = 0; k < 4; ++k) {   // hi.whi | hi.wlo
+              tc::wgmma_f16<N2>(acc0, a0 + 2 * k, w0 + 2 * k, (tap | k) ? 1u : 0u);
+              tc::wgmma_f16<N2>(acc1, a0 + HALF + 2 * k, w0 + 2 * k, (tap | k) ? 1u : 0u);
+            }
 #pragma unroll
-              for (int k = 0; k < 4; ++k) tc::umma_f16(d, a1 + 2 * k, w0 + 2 * k, idesc, 1u);                    // lo.whi
-            } else {
+            for (int k = 0; k < 4; ++k) {   // lo.whi
+              tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc0), a1 + 2 * k, w0 + 2 * k, 1u);
+              tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc1), a1 + HALF + 2 * k, w0 + 2 * k, 1u);
+            }
+          } else {
 #pragma unroll
-              for (int k = 0; k < C::KSTEPS; ++k) {   // [hi|lo].[[whi|whi];[wlo|0]]; the lo K-steps of 128-byte rows skip the zero block
-                const bool lo_half = (C::ROWB == 128) && (k >= C::KSTEPS / 2);
-                tc::umma_f16(d, a0 + 2 * k, w0 + 2 * k, lo_half ? idesc : idesc2, (tap | k) ? 1u : 0u);
+            for (int k = 0; k < C::KSTEPS; ++k) {   // [hi|lo].[[whi|whi];[wlo|0]]; the lo K-steps of 128-byte rows skip the zero block
+              const bool lo_half = (C::ROWB == 128) && (k >= C::KSTEPS / 2);
+              if (lo_half) {
+                tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc0), a0 + 2 * k, w0 + 2 * k, 1u);
+                tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc1), a0 + HALF + 2 * k, w0 + 2 * k, 1u);
+              } else {
+                tc::wgmma_f16<N2>(acc0, a0 + 2 * k, w0 + 2 * k, (tap | k) ? 1u : 0u);
+                tc::wgmma_f16<N2>(acc1, a0 + HALF + 2 * k, w0 + 2 * k, (tap | k) ? 1u : 0u);
               }
             }
           }
-          tc::umma_commit(&a_empty[s]);
         }
-        tc::umma_commit(&acc_full[a]);
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&a_empty[s]);   // this warp's reads of the stage are complete
       }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue ----------------
-    // two epilogue groups (warps 2-5, 6-9) take alternate tiles: the epilogue of a thin tile (TMEM load latency, global
-    // stores, skip-branch loads) is longer than its handful of UMMAs, so two tiles are drained concurrently
-    const int q = warp & 3, eg = (warp - 2) >> 2;
-    const int r = q * 32 + lane;                 // pixel of the tile = TMEM lane
-    const int ph_ = r >> P.tw_log2, pw_ = r & (TW - 1);
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-      if ((int)(tcount & 1) != eg) continue;
-      const int a = tcount % NACC;
+      // ---------------- epilogue ----------------
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      tc::mbar_wait(&acc_full[a], (tcount / NACC) & 1);
-      tc::tc_fence_after();
-      uint32_t v[2 * NOUT];
-      __syncwarp();
+      uint32_t v[N2];
 #pragma unroll
-      for (int c = 0; c < 2 * NOUT / 32; ++c) {
+      for (int c = 0; c < N2 / 32; ++c) {
         uint32_t t[32];
-        tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * C::ACC_COLS + c * 32, t);
+        tc::acc_rows<32>(sStg, acc0, acc1, c * 32, r, 1, t);
 #pragma unroll
         for (int j = 0; j < 32; ++j) v[c * 32 + j] = t[j];
       }
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[a]);   // TMEM buffer is free again: the stores below overlap the next MMAs
       if (y < P.H && x < P.W) {
         const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
         float o[NOUT];
@@ -263,12 +240,6 @@ __global__ void __launch_bounds__(CT_THREADS2, 1) conv_tc_kernel(const __grid_co
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, C::TMEM_COLS);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -278,7 +249,7 @@ __global__ void __launch_bounds__(CT_THREADS2, 1) conv_tc_kernel(const __grid_co
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int C128_WBOX = 64 * 128;
 constexpr int C128_STAGE = 4 * CT_ABOX + 4 * C128_WBOX;   // 96 KB
-constexpr size_t C128_SMEM = 1024 + 2 * (size_t)C128_STAGE + 768;
+constexpr size_t C128_SMEM = 1024 + 2 * (size_t)C128_STAGE + tc::STG_BYTES + 768;
 
 template <int KS>
 __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_constant__ ConvTcParams P) {
@@ -286,13 +257,11 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sS = base;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + NS * (size_t)C128_STAGE);
+  float* sStg = reinterpret_cast<float*>(base + NS * (size_t)C128_STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + NS * (size_t)C128_STAGE + tc::STG_BYTES);
   uint64_t* s_full = bars;           // [NS]
   uint64_t* s_empty = bars + NS;     // [NS]
-  uint64_t* acc_full = bars + 2 * NS;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* sBias = reinterpret_cast<float*>(tmem_slot + 2);
+  float* sBias = reinterpret_cast<float*>(bars + 2 * NS);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int TW = 1 << P.tw_log2, TH = 128 >> P.tw_log2;
@@ -303,29 +272,18 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
   const int co0 = nt * NOUT;
 
   if (threadIdx.x < NOUT) sBias[threadIdx.x] = __ldg(P.bias + co0 + threadIdx.x);
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
     for (int i = 0; i < NS; ++i) {
       tc::mbar_init(&s_full[i], 1);
-      tc::mbar_init(&s_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 4);
+      tc::mbar_init(&s_empty[i], 4);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, 256);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (tc::elect_one()) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -347,58 +305,48 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, NOUT);
-      constexpr uint32_t idesc2 = tc::make_idesc(/*F16*/ 0, 128, 2 * NOUT);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-        const int a = tcount & 1;
-        tc::mbar_wait(&acc_empty[a], ((tcount >> 1) & 1) ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem + a * 2 * NOUT;
-        for (int tap = 0; tap < TAPS; ++tap, ++it) {
-          const int s = it % NS;
-          tc::mbar_wait(&s_full[s], (it / NS) & 1);
-          tc::tc_fence_after();
-          const uint32_t sa = tc::smem_u32(sS + (size_t)s * C128_STAGE), sw = sa + 4 * CT_ABOX;
-#pragma unroll
-          for (int kb = 0; kb < 2; ++kb) {
-            const uint64_t ahi = tc::make_desc_sw128(sa + kb * CT_ABOX, 1024), alo = tc::make_desc_sw128(sa + (2 + kb) * CT_ABOX, 1024);
-            const uint64_t whi = tc::make_desc_sw128(sw + (2 * kb) * C128_WBOX, 1024);   // also [whi_kb ; wlo_kb] with N = 128
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16(d, ahi + 2 * k, whi + 2 * k, idesc2, (tap | kb | k) ? 1u : 0u);  // hi.whi | hi.wlo
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16(d, alo + 2 * k, whi + 2 * k, idesc, 1u);                         // lo.whi
-          }
-          tc::umma_commit(&s_empty[s]);
-        }
-        tc::umma_commit(&acc_full[a]);
-      }
-    }
-    __syncwarp();
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
+    constexpr uint32_t HALF = (64 * 128) >> 4;   // descriptor offset of rows 64-127
+    const int r = threadIdx.x;
     const int ph_ = r >> P.tw_log2, pw_ = r & (TW - 1);
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-      const int a = tcount & 1;
+    float acc0[NOUT], acc1[NOUT];                 // rows 0-63 / 64-127, 2*NOUT columns each
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      for (int tap = 0; tap < TAPS; ++tap, ++it) {
+        const int s = it % NS;
+        tc::mbar_wait(&s_full[s], (it / NS) & 1);
+        tc::wgmma_fence();
+        const uint32_t sa = tc::smem_u32(sS + (size_t)s * C128_STAGE), sw = sa + 4 * CT_ABOX;
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+          const uint64_t ahi = tc::make_desc_sw128(sa + kb * CT_ABOX, 1024), alo = tc::make_desc_sw128(sa + (2 + kb) * CT_ABOX, 1024);
+          const uint64_t whi = tc::make_desc_sw128(sw + (2 * kb) * C128_WBOX, 1024);   // also [whi_kb ; wlo_kb] with N = 128
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {   // hi.whi | hi.wlo
+            tc::wgmma_f16<2 * NOUT>(acc0, ahi + 2 * k, whi + 2 * k, (tap | kb | k) ? 1u : 0u);
+            tc::wgmma_f16<2 * NOUT>(acc1, ahi + HALF + 2 * k, whi + 2 * k, (tap | kb | k) ? 1u : 0u);
+          }
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {   // lo.whi
+            tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc0), alo + 2 * k, whi + 2 * k, 1u);
+            tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc1), alo + HALF + 2 * k, whi + 2 * k, 1u);
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&s_empty[s]);
+      }
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      tc::mbar_wait(&acc_full[a], (tcount >> 1) & 1);
-      tc::tc_fence_after();
       uint32_t v0[32], v1[32], v2[32], v3[32];
-      __syncwarp();
-      tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * 2 * NOUT, v0);
-      tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * 2 * NOUT + 32, v1);
-      tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * 2 * NOUT + 64, v2);
-      tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * 2 * NOUT + 96, v3);
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[a]);
+      tc::acc_rows<32>(sStg, acc0, acc1, 0, r, 1, v0);
+      tc::acc_rows<32>(sStg, acc0, acc1, 32, r, 1, v1);
+      tc::acc_rows<32>(sStg, acc0, acc1, 64, r, 1, v2);
+      tc::acc_rows<32>(sStg, acc0, acc1, 96, r, 1, v3);
       if (y < P.H && x < P.W) {
         const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
         float o[NOUT];
@@ -416,12 +364,6 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
         }
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 256);
   }
 }
 
@@ -598,7 +540,7 @@ template <int KS, int CINP, int NOUT>
 static int launch_tc_cfg(const ConvTcParams& P, int grid, cudaStream_t st) {
   using C = ConvTcCfg<KS, CINP, NOUT>;
   XF_DYN_SMEM((conv_tc_kernel<KS, CINP, NOUT>), C::SMEM);
-  conv_tc_kernel<KS, CINP, NOUT><<<grid, CT_THREADS2, C::SMEM, st>>>(P);
+  conv_tc_kernel<KS, CINP, NOUT><<<grid, CT_THREADS, C::SMEM, st>>>(P);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -1,4 +1,4 @@
-// 3x3 / stride-1 convolution on tcgen05 with HALO-PATCH operand reuse.
+// 3x3 / stride-1 convolution on the Hopper tensor cores (wgmma) with HALO-PATCH operand reuse.
 //
 // conv_tc_kernel re-reads the input patch once per tap (9x the activation bytes through L2).  Here the haloed patch
 // (TH+2) x (TW+2) pixels is loaded ONCE per tile by a single 4-D TMA box into a 128B-swizzled K-major array whose rows
@@ -7,8 +7,8 @@
 // then the A operand of tap (dy,dx) is the SAME array shifted by a constant number of rows:
 //      row(m, tap) = m + dy * PW + dx
 // i.e. the tap is selected by advancing the shared-memory matrix descriptor's start address by (dy*PW+dx)*128 bytes
-// (not 1024-aligned in general; measured on B200: the 128B swizzle is applied on physical address bits, so the shifted
-// descriptor keeps base_offset = 0 -- see tests/test_gpu_conv_halo.py, which checks both settings).
+// (not 1024-aligned in general; the 128B swizzle is applied on physical address bits, so the shifted descriptor keeps
+// base_offset = 0 -- see tests/test_gpu_conv_halo.py, which checks both settings).
 // TH * PW <= 128, so a tile yields TH*TW valid pixels out of 128 MMA rows (TW = 40: 120/128).
 #include <cuda_fp16.h>
 
@@ -17,27 +17,20 @@
 
 namespace xf {
 
-constexpr int CH_THREADS = 320;   // warp 0 TMA, warp 1 MMA, epilogue groups warps 2-5 / 6-9 on alternate tiles
+constexpr int CH_THREADS = 160;   // warps 0-3: wgmma + epilogue warpgroup, warp 4: TMA producer
 constexpr int CH_PATCH_BYTES = 34816;   // CINP=32: >= (2*PW + 2 + 128) * 128 for PW <= 66, multiple of 1024
-constexpr int CH_PATCH64_BYTES = 27648; // CINP=64: PW <= 42 (TW <= 40): 214 rows x 128 B, so that THREE buffers fit beside the weights
+constexpr int CH_PATCH64_BYTES = 27648; // CINP=64: PW <= 42 (TW <= 40): 214 rows x 128 B
 
 template <int CINP, int NOUT>
 struct HaloCfg {
   static constexpr int ROWB = (CINP == 8) ? 32 : 128;     // bytes per operand row: [hi(8)|lo(8)] halves, or 64 halves
-  static constexpr int KSTEPS = ROWB / 32;                // UMMA K = 16 halves = 32 B
+  static constexpr int KSTEPS = ROWB / 32;                // wgmma K = 16 halves = 32 B
   static constexpr int W_GROUP = NOUT * ROWB;
   static constexpr size_t W_BYTES = (size_t)9 * 2 * W_GROUP;
-  // patch buffers: CINP=32 -> 4-deep ring over tiles; CINP=64 -> 3-deep ring over the sequence hi(t), lo(t), hi(t+1), ...
-  static constexpr int NP = (CINP == 64) ? 3 : (CINP == 32 ? 4 : 16);
+  // patch buffers: CINP=32 -> 4-deep ring over tiles; CINP=64 -> hi and lo buffer (the 144 KB of weights leave no room for more)
+  static constexpr int NP = (CINP == 64) ? 2 : (CINP == 32 ? 4 : 16);
   static constexpr int PB = (CINP == 64) ? CH_PATCH64_BYTES : (CINP == 32 ? CH_PATCH_BYTES : CH_PATCH_BYTES / 4);
-  static constexpr size_t SMEM = 1024 + W_BYTES + NP * (size_t)PB + 1024;
-  // accumulator per buffer: columns [0,NOUT) = terms against whi, [NOUT,2*NOUT) = terms against wlo (one UMMA with
-  // N = 2*NOUT reads the activation operand once for both weight groups); the epilogue adds the two halves.
-  static constexpr int ACC_COLS = 2 * NOUT;
-  // accumulator ring: the MMA -> epilogue -> MMA round trip (commit, mbarrier wake-up, tcgen05.ld, arrive) costs ~1-2k cycles,
-  // far more than the MMAs of a thin tile, so several tiles are kept in flight in TMEM (512 columns available).
-  static constexpr int NACC = (512 / ACC_COLS) > 8 ? 8 : (512 / ACC_COLS);
-  static constexpr int TMEM_COLS = NACC * ACC_COLS < 32 ? 32 : NACC * ACC_COLS;
+  static constexpr size_t SMEM = 1024 + W_BYTES + NP * (size_t)PB + tc::STG_BYTES + 1024;
 };
 
 struct HaloParams {
@@ -52,7 +45,7 @@ struct HaloParams {
   int f32_c, n_real;
   int relu;
   FastDiv div_img, div_x;
-  int desc_mode;      // 0 (default, correct on B200): base_offset = 0; 1: base_offset = (addr >> 7) & 7 (bring-up experiment)
+  int desc_mode;      // 0 (default): base_offset = 0; 1: base_offset = (addr >> 7) & 7 (bring-up experiment)
 };
 
 __device__ __forceinline__ uint64_t make_desc_sw128_at(uint32_t smem_addr, uint32_t sbo_bytes, int mode) {
@@ -74,15 +67,12 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
   unsigned char* sP = base + C::W_BYTES;                     // patch buffers
   constexpr int NP = C::NP;
   constexpr int PB = C::PB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + NP * PB);
+  float* sStg = reinterpret_cast<float*>(base + C::W_BYTES + NP * PB);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + NP * PB + tc::STG_BYTES);
   uint64_t* w_full = bars;
   uint64_t* p_full = bars + 1;            // [NP]
   uint64_t* p_empty = bars + 1 + NP;      // [NP]
-  constexpr int NACC = C::NACC;
-  uint64_t* acc_full = bars + 1 + 2 * NP; // [NACC]
-  uint64_t* acc_empty = acc_full + NACC;  // [NACC]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + NACC);
-  float* sBias = reinterpret_cast<float*>(tmem_slot + 2);
+  float* sBias = reinterpret_cast<float*>(bars + 1 + 2 * NP);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_x = (P.W + P.TW - 1) / P.TW, tiles_y = (P.H + P.TH - 1) / P.TH;
@@ -92,33 +82,22 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
   const uint32_t patch_tx = (uint32_t)(P.TH + 2) * P.PW * ROWB;
 
   if (threadIdx.x < NOUT) sBias[threadIdx.x] = (threadIdx.x < P.n_real) ? __ldg(P.bias + threadIdx.x) : 0.f;
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
     tc::mbar_init(w_full, 1);
     for (int i = 0; i < NP; ++i) {
       tc::mbar_init(&p_full[i], 1);
-      tc::mbar_init(&p_empty[i], 1);
-    }
-    for (int i = 0; i < NACC; ++i) {
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 4);
+      tc::mbar_init(&p_empty[i], 4);   // one arrival per consumer warp
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, C::TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  // CINP = 64: buffer 0 = hi patch, buffer 1 = lo patch of the SAME tile (each single-buffered; the hi-only MMAs of a
-  //            tile run first so the next tile's hi patch can stream in while the lo MMAs run, and vice versa).
-  // CINP = 32: a ring of NP buffers over tiles (rows are [hi(32)|lo(32)]): the producer runs up to NP-1 tiles ahead.
-  if (warp == 0) {
+  // CINP = 64: buffer 0 = hi patch, buffer 1 = lo patch of the SAME tile (the hi MMAs of a tile run first, so the next tile's
+  //            hi patch streams in while the lo MMAs and the epilogue run).
+  // CINP = 32 / 8: a ring of NP buffers over tiles (rows are [hi|lo]): the producer runs up to NP-1 tiles ahead.
+  if (warp == 4) {
     if (tc::elect_one()) {
       tc::mbar_expect_tx(w_full, (uint32_t)C::W_BYTES);
       for (int i = 0; i < 18; ++i) tc::tma_load_2d(sW + (size_t)i * C::W_GROUP, &P.wmap, w_full, 0, i * NOUT);
@@ -145,96 +124,106 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, NOUT);        // against one weight group
-      constexpr uint32_t idesc2 = tc::make_idesc(/*F16*/ 0, 128, 2 * NOUT);   // against [group0 ; group1] stacked along N
-      tc::mbar_wait(w_full, 0);
-      const uint32_t w_base = tc::smem_u32(sW);
-      uint32_t tcount = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-        const int a = tcount % NACC;
-        tc::mbar_wait(&acc_empty[a], ((tcount / NACC) & 1) ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem + a * C::ACC_COLS;
-        if (CINP == 64) {
-          const uint32_t li_hi = 2 * tcount, li_lo = 2 * tcount + 1;
-          const int s_hi = li_hi % NP, s_lo = li_lo % NP;
-          const uint32_t hi_base = tc::smem_u32(sP) + (uint32_t)s_hi * PB, lo_base = tc::smem_u32(sP) + (uint32_t)s_lo * PB;
-          tc::mbar_wait(&p_full[s_hi], (li_hi / NP) & 1);
-          tc::tc_fence_after();
-          for (int tap = 0; tap < 9; ++tap) {
-            const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * 128u;
-            const uint64_t ahi = make_desc_sw128_at(hi_base + shift, 1024, P.desc_mode);
-            const uint64_t wboth = tc::make_desc_sw128(w_base + (uint32_t)(tap * 2) * C::W_GROUP, 1024);   // [whi ; wlo], N = 128
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16(d, ahi + 2 * k, wboth + 2 * k, idesc2, (tap | k) ? 1u : 0u);   // hi.whi | hi.wlo
-          }
-          tc::umma_commit(&p_empty[s_hi]);         // hi patch buffer may be refilled once these MMAs retire
-          tc::mbar_wait(&p_full[s_lo], (li_lo / NP) & 1);
-          tc::tc_fence_after();
-          for (int tap = 0; tap < 9; ++tap) {
-            const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * 128u;
-            const uint64_t alo = make_desc_sw128_at(lo_base + shift, 1024, P.desc_mode);
-            const uint64_t whi = tc::make_desc_sw128(w_base + (uint32_t)(tap * 2) * C::W_GROUP, 1024);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16(d, alo + 2 * k, whi + 2 * k, idesc, 1u);
-          }
-          tc::umma_commit(&p_empty[s_lo]);
-        } else {
-          const int s = tcount % NP;
-          const uint32_t p_base = tc::smem_u32(sP) + (uint32_t)s * PB;
-          tc::mbar_wait(&p_full[s], (tcount / NP) & 1);
-          tc::tc_fence_after();
-          for (int tap = 0; tap < 9; ++tap) {
-            const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * (uint32_t)ROWB;
-            const uint64_t a0 = make_desc_rows_at<ROWB>(p_base + shift, P.desc_mode);
-            const uint64_t wboth = tc::make_desc_rows<ROWB>(w_base + (uint32_t)(tap * 2) * C::W_GROUP);
-#pragma unroll
-            for (int k = 0; k < KSTEPS; ++k) {   // [hi|lo] . [[whi|whi] ; [wlo|0]]  ->  cols [0,N): hi.whi + lo.whi, cols [N,2N): hi.wlo
-              // 128-byte rows: K-steps 0,1 are the hi channels, 2,3 the lo channels, whose [wlo|0] rows multiply by zero -- those
-              // K-steps run at N = NOUT against the [whi|whi] rows only (a quarter less tensor work, 1 KB less operand traffic each)
-              const bool lo_half = (ROWB == 128) && (k >= KSTEPS / 2);
-              tc::umma_f16(d, a0 + 2 * k, wboth + 2 * k, lo_half ? idesc : idesc2, (tap | k) ? 1u : 0u);
-            }
-          }
-          tc::umma_commit(&p_empty[s]);
-        }
-        tc::umma_commit(&acc_full[a]);
-      }
-    }
-    __syncwarp();
   } else {
-    const int q = warp & 3, eg = (warp - 2) >> 2;   // two epilogue groups on alternate tiles (see conv_tc.cu)
-    const int m = q * 32 + lane;
+    constexpr int N2 = 2 * NOUT;
+    constexpr uint32_t HALF = 64u * ROWB;          // bytes: rows 64-127 of the GEMM
+    const int m = threadIdx.x;                     // GEMM row of this thread = patch-pitch pixel
     const int mh = m / P.PW, mw = m - mh * P.PW;
     const bool lane_ok = (mh < P.TH) && (mw < P.TW);
+    float acc0[NOUT], acc1[NOUT];
+    const uint32_t w_base = tc::smem_u32(sW);
+    tc::mbar_wait(w_full, 0);
     uint32_t tcount = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-      if ((int)(tcount & 1) != eg) continue;
-      const int a = tcount % NACC;
+      if (CINP == 64) {
+        const uint32_t li_hi = 2 * tcount, li_lo = 2 * tcount + 1;
+        const int s_hi = li_hi % NP, s_lo = li_lo % NP;
+        const uint32_t hi_base = tc::smem_u32(sP) + (uint32_t)s_hi * PB, lo_base = tc::smem_u32(sP) + (uint32_t)s_lo * PB;
+        tc::mbar_wait(&p_full[s_hi], (li_hi / NP) & 1);
+        tc::wgmma_fence();
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * 128u;
+          const uint64_t ahi = make_desc_sw128_at(hi_base + shift, 1024, P.desc_mode);
+          const uint64_t ahi1 = make_desc_sw128_at(hi_base + shift + HALF, 1024, P.desc_mode);
+          const uint64_t wboth = tc::make_desc_sw128(w_base + (uint32_t)(tap * 2) * C::W_GROUP, 1024);   // [whi ; wlo], N = 128
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {   // hi.whi | hi.wlo
+            tc::wgmma_f16<N2>(acc0, ahi + 2 * k, wboth + 2 * k, (tap | k) ? 1u : 0u);
+            tc::wgmma_f16<N2>(acc1, ahi1 + 2 * k, wboth + 2 * k, (tap | k) ? 1u : 0u);
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&p_empty[s_hi]);   // hi patch buffer may be refilled
+        tc::mbar_wait(&p_full[s_lo], (li_lo / NP) & 1);
+        tc::wgmma_fence();
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * 128u;
+          const uint64_t alo = make_desc_sw128_at(lo_base + shift, 1024, P.desc_mode);
+          const uint64_t alo1 = make_desc_sw128_at(lo_base + shift + HALF, 1024, P.desc_mode);
+          const uint64_t whi = tc::make_desc_sw128(w_base + (uint32_t)(tap * 2) * C::W_GROUP, 1024);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {   // lo.whi
+            tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc0), alo + 2 * k, whi + 2 * k, 1u);
+            tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc1), alo1 + 2 * k, whi + 2 * k, 1u);
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&p_empty[s_lo]);
+      } else {
+        const int s = tcount % NP;
+        const uint32_t p_base = tc::smem_u32(sP) + (uint32_t)s * PB;
+        tc::mbar_wait(&p_full[s], (tcount / NP) & 1);
+        tc::wgmma_fence();
+        for (int tap = 0; tap < 9; ++tap) {
+          const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * (uint32_t)ROWB;
+          const uint64_t a0 = make_desc_rows_at<ROWB>(p_base + shift, P.desc_mode);
+          const uint64_t a1 = make_desc_rows_at<ROWB>(p_base + shift + HALF, P.desc_mode);
+          const uint64_t wboth = tc::make_desc_rows<ROWB>(w_base + (uint32_t)(tap * 2) * C::W_GROUP);
+#pragma unroll
+          for (int k = 0; k < KSTEPS; ++k) {   // [hi|lo] . [[whi|whi] ; [wlo|0]]  ->  cols [0,N): hi.whi + lo.whi, cols [N,2N): hi.wlo
+            // 128-byte rows: K-steps 0,1 are the hi channels, 2,3 the lo channels, whose [wlo|0] rows multiply by zero -- those
+            // K-steps run at N = NOUT against the [whi|whi] rows only
+            const bool lo_half = (ROWB == 128) && (k >= KSTEPS / 2);
+            if (lo_half) {
+              tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc0), a0 + 2 * k, wboth + 2 * k, 1u);
+              tc::wgmma_f16<NOUT>(tc::acc_head<NOUT>(acc1), a1 + 2 * k, wboth + 2 * k, 1u);
+            } else {
+              tc::wgmma_f16<N2>(acc0, a0 + 2 * k, wboth + 2 * k, (tap | k) ? 1u : 0u);
+              tc::wgmma_f16<N2>(acc1, a1 + 2 * k, wboth + 2 * k, (tap | k) ? 1u : 0u);
+            }
+          }
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&p_empty[s]);
+      }
+      // ---------------- epilogue ----------------
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * P.TH + mh, x = tx_ * P.TW + mw;
-      tc::mbar_wait(&acc_full[a], (tcount / NACC) & 1);
-      tc::tc_fence_after();
-      uint32_t v[2 * NOUT];
-      __syncwarp();
+      uint32_t v[N2];
       if constexpr (NOUT == 8) {
-        tc::tmem_ld_32x16(tmem + ((uint32_t)(q * 32) << 16) + a * C::ACC_COLS, v);
+        tc::acc_rows<16>(sStg, acc0, acc1, 0, m, 1, v);
       } else {
 #pragma unroll
-        for (int c = 0; c < 2 * NOUT / 32; ++c) {
+        for (int c = 0; c < N2 / 32; ++c) {
           uint32_t t[32];
-          tc::tmem_ld_32x32(tmem + ((uint32_t)(q * 32) << 16) + a * C::ACC_COLS + c * 32, t);
+          tc::acc_rows<32>(sStg, acc0, acc1, c * 32, m, 1, t);
 #pragma unroll
           for (int j = 0; j < 32; ++j) v[c * 32 + j] = t[j];
         }
       }
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[a]);
       if (lane_ok && y < P.H && x < P.W) {
         const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
         float o[NOUT];
@@ -252,12 +241,6 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, C::TMEM_COLS);
-  }
 }
 
 // tile geometry: TW <= 64 (PW <= 66), TH = 128 / PW; minimise MMA rows spent per valid output pixel
@@ -273,8 +256,8 @@ static void pick_halo_tile(int H, int W, int tw_max, int& TW, int& TH) {
   }
 }
 
-int g_halo_desc_mode = 0;   // measured on B200: the UMMA swizzle is a function of the physical shared-memory address, so a
-                            // start address shifted by whole 128-byte rows needs base_offset = 0 (mode 1 gives wrong results)
+int g_halo_desc_mode = 0;   // the wgmma swizzle is a function of the physical shared-memory address, so a start address
+                            // shifted by whole 128-byte rows needs base_offset = 0 (mode 1 gives wrong results)
 
 // same contract as launch_conv_tc, for 3x3 stride-1 layers with (CINP,NOUT) in {(64,64), (32,32)}
 int launch_conv_tc_halo(const xfeat_ctx* ctx, int layer, const __half* in_split, int B, int H, int W, __half* out_split,

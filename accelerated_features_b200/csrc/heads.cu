@@ -148,15 +148,13 @@ __global__ void __launch_bounds__(KPT_WARPS * 32) kpt_softmax_kernel(const float
 
 // Same fusion, but x3 / x4 / x5 arrive as split fp16 [hi(64) | lo(64)] (x = hi + lo) straight from the tensor-core layers, so
 // block3.2 / block4.2 / block5.3 need not write a second, fp32 copy of their output.
-// 16 channels per thread: 256-bit loads (LDG.E.ENL2.256) of the hi and lo halves, 256-bit stores: half the instructions per byte
-// of the 128-bit version (the kernel is issue-bound on its 18 loads per thread).
+// 16 channels per thread: 32 bytes of the hi and of the lo halves per load call (two 128-bit read-only loads each).
 struct F16v {
   float v[16];
 };
 __device__ __forceinline__ void ld_v8_nc(const void* p, uint32_t (&r)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 __device__ __forceinline__ F16v ld_split16(const __half* __restrict__ base, int64_t pix, int c16) {
   uint32_t hw[8], lw[8];

@@ -3,13 +3,14 @@
 // Each layer is one launch of a persistent split-fp16 GEMM  Y[rows x N] = X[rows x K] . W[N x K]^T  over ALL coarse matches of
 // the batch at once (rows = sum of the per-pair match counts, read from device memory: tiles past the live rows are never
 // scheduled).  Operands are split as everywhere in this library: x = hi + lo (fp16), w * 2^k = whi + wlo,
-//      y = (hi.whi + hi.wlo + lo.whi) * 2^-k + b          (fp32 accumulation in TMEM)
+//      y = (hi.whi + hi.wlo + lo.whi) * 2^-k + b          (fp32 accumulation in registers)
 // so the result is fp32-equivalent (tests: 1e-3 of the logit range; refined coordinates 2e-3 px).  Activations travel between
 // the layers already split, rows of [hi(K) | lo(K)] halves, written by the producing epilogue.
-//   warp 0: TMA producer, one 64-channel K block per stage {A hi, A lo, W hi, W lo};  warp 1: MMA issuer: per K block
-//   4 x UMMA(128 x 2NT x 16) hi.[whi ; wlo] + 4 x UMMA(128 x NT x 16) lo.whi;  warps 2-5: epilogue (bias, ReLU, split, 256-bit
-//   stores), accumulators double buffered in TMEM.  Weights (1 MB per 512 x 512 layer) stream from L2; an n-fastest tile
-//   order keeps the A tile of a row block L2-resident across its N tiles.
+//   warp 4: TMA producer, one 64-channel K block per stage {A hi, A lo, W hi, W lo};  warps 0-3: one warpgroup that issues, per
+//   K block and 64-row slab, 4 x wgmma(64 x 2NT x 16) hi.[whi ; wlo] + 4 x wgmma(64 x NT x 16) lo.whi, then runs the epilogue
+//   (bias, ReLU, split, one row per thread).  NT = 64: the 2 x 128 accumulator columns of both slabs fill 128 registers per
+//   thread.  Weights (1 MB per 512 x 512 layer) stream from L2; an n-fastest tile order keeps the A tile of a row block
+//   L2-resident across its N tiles.
 // Replaces the five fp32 CUDA-core launches of round 1 (refine.cu); the fp32 path stays as xfeat_set_conv_impl(0).
 #include <cuda_fp16.h>
 
@@ -20,16 +21,14 @@
 
 namespace xf {
 
-constexpr int ML_THREADS = 192, ML_BOX = 128 * 128;   // 128 rows x 64 halves
+constexpr int ML_THREADS = 160, ML_BOX = 128 * 128;   // 128 rows x 64 halves
 
 template <int NT>
 struct MlpCfg {
   static constexpr int W_BOX = NT * 128;                         // NT rows x 64 halves
   static constexpr int STAGE = 2 * ML_BOX + 2 * W_BOX;           // A hi, A lo, W hi, W lo
-  static constexpr int NS = (NT == 128) ? 3 : 4;
-  static constexpr size_t SMEM = 1024 + (size_t)NS * STAGE + 256;
-  static constexpr int ACC_COLS = 2 * NT;
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;                 // double buffered
+  static constexpr int NS = 4;
+  static constexpr size_t SMEM = 1024 + (size_t)NS * STAGE + tc::STG_BYTES + 256;
 };
 
 struct MlpParams {
@@ -51,12 +50,10 @@ __global__ void __launch_bounds__(ML_THREADS, 1) mlp_gemm_kernel(const __grid_co
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sS = base;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (size_t)C::NS * C::STAGE);
+  float* sStg = reinterpret_cast<float*>(base + (size_t)C::NS * C::STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (size_t)C::NS * C::STAGE + tc::STG_BYTES);
   uint64_t* s_full = bars;                 // [NS]
   uint64_t* s_empty = bars + C::NS;        // [NS]
-  uint64_t* acc_full = bars + 2 * C::NS;   // [2]
-  uint64_t* acc_empty = acc_full + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rows = P.n_live ? min(__ldg(P.n_live), P.rows_cap) : P.rows_cap;
@@ -64,29 +61,18 @@ __global__ void __launch_bounds__(ML_THREADS, 1) mlp_gemm_kernel(const __grid_co
   const int total = m_tiles * P.n_tiles;
   const int KB = P.K / 64;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
     for (int i = 0; i < C::NS; ++i) {
       tc::mbar_init(&s_full[i], 1);
-      tc::mbar_init(&s_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 4);
+      tc::mbar_init(&s_empty[i], 4);   // one arrival per consumer warp
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, C::TMEM_COLS);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (tc::elect_one()) {
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
@@ -104,57 +90,44 @@ __global__ void __launch_bounds__(ML_THREADS, 1) mlp_gemm_kernel(const __grid_co
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc1 = tc::make_idesc(/*F16*/ 0, 128, NT);
-      constexpr uint32_t idesc2 = tc::make_idesc(/*F16*/ 0, 128, 2 * NT);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++tcount) {
-        const int a = tcount & 1;
-        tc::mbar_wait(&acc_empty[a], ((tcount >> 1) & 1) ^ 1);
-        tc::tc_fence_after();
-        const uint32_t d = tmem + a * C::ACC_COLS;
-        for (int kb = 0; kb < KB; ++kb, ++it) {
-          const int s = it % C::NS;
-          tc::mbar_wait(&s_full[s], (it / C::NS) & 1);
-          tc::tc_fence_after();
-          const uint32_t sa = tc::smem_u32(sS + (size_t)s * C::STAGE);
-          const uint64_t ahi = tc::make_desc_sw128(sa, 1024), alo = tc::make_desc_sw128(sa + ML_BOX, 1024);
-          const uint64_t w = tc::make_desc_sw128(sa + 2 * ML_BOX, 1024);     // [whi ; wlo]: 2 NT rows, or whi alone: NT rows
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_f16(d, ahi + 2 * k, w + 2 * k, idesc2, (kb | k) ? 1u : 0u);   // hi.whi | hi.wlo
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_f16(d, alo + 2 * k, w + 2 * k, idesc1, 1u);                   // lo.whi
-          tc::umma_commit(&s_empty[s]);
-        }
-        tc::umma_commit(&acc_full[a]);
-      }
-    }
-    __syncwarp();
   } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < total; tile += gridDim.x, ++tcount) {
-      const int a = tcount & 1;
+    constexpr uint32_t HALF = (64 * 128) >> 4;   // descriptor offset of rows 64-127
+    const int r = threadIdx.x;
+    float acc0[NT], acc1[NT];                     // rows 0-63 / 64-127, 2*NT columns each
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
       const int m = tile / P.n_tiles, nt = tile - m * P.n_tiles;
+      for (int kb = 0; kb < KB; ++kb, ++it) {
+        const int s = it % C::NS;
+        tc::mbar_wait(&s_full[s], (it / C::NS) & 1);
+        tc::wgmma_fence();
+        const uint32_t sa = tc::smem_u32(sS + (size_t)s * C::STAGE);
+        const uint64_t ahi = tc::make_desc_sw128(sa, 1024), alo = tc::make_desc_sw128(sa + ML_BOX, 1024);
+        const uint64_t w = tc::make_desc_sw128(sa + 2 * ML_BOX, 1024);     // [whi ; wlo]: 2 NT rows, or whi alone: NT rows
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {   // hi.whi | hi.wlo
+          tc::wgmma_f16<2 * NT>(acc0, ahi + 2 * k, w + 2 * k, (kb | k) ? 1u : 0u);
+          tc::wgmma_f16<2 * NT>(acc1, ahi + HALF + 2 * k, w + 2 * k, (kb | k) ? 1u : 0u);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {   // lo.whi
+          tc::wgmma_f16<NT>(tc::acc_head<NT>(acc0), alo + 2 * k, w + 2 * k, 1u);
+          tc::wgmma_f16<NT>(tc::acc_head<NT>(acc1), alo + HALF + 2 * k, w + 2 * k, 1u);
+        }
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&s_empty[s]);
+      }
       const int row = m * 128 + r;
       const bool live = row < rows;
-      tc::mbar_wait(&acc_full[a], (tcount >> 1) & 1);
-      tc::tc_fence_after();
-      const uint32_t tb = tmem + ((uint32_t)(q * 32) << 16) + a * C::ACC_COLS;
-#pragma unroll 1
+#pragma unroll
       for (int c0 = 0; c0 < NT; c0 += 32) {
         uint32_t v0[32], v1[32];
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + c0, v0);
-        tc::tmem_ld_32x32(tb + NT + c0, v1);
-        tc::tmem_ld_wait();
-        if (c0 + 32 == NT) {             // last chunk read: the accumulator buffer goes back to the MMA warp
-          tc::tc_fence_before();
-          __syncwarp();
-          if (lane == 0) tc::mbar_arrive(&acc_empty[a]);
-        }
+        tc::acc_rows<32>(sStg, acc0, acc1, c0, r, 1, v0);
+        tc::acc_rows<32>(sStg, acc0, acc1, NT + c0, r, 1, v1);
         const int n0 = nt * NT + c0;
         if (live && n0 < P.N) {
           float o[32];
@@ -172,12 +145,6 @@ __global__ void __launch_bounds__(ML_THREADS, 1) mlp_gemm_kernel(const __grid_co
         }
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, C::TMEM_COLS);
   }
 }
 
@@ -243,7 +210,7 @@ static int mlp_map(CUtensorMap* m, const void* ptr, uint64_t row_halves, uint64_
 static int launch_mlp_layer(const xfeat_ctx* ctx, int i, const __half* x_split, int rows_cap, const int* n_live, __half* out_split,
                             float* out_f32, cudaStream_t st) {
   const LayerSpec& sp = kLayers[kMlpLayers[i]];
-  const int NT = (sp.cout % 128 == 0) ? 128 : 64;
+  constexpr int NT = 64;
   const int npad = (sp.cout + 63) / 64 * 64;
   MlpParams P;
   int rc;
@@ -257,13 +224,8 @@ static int launch_mlp_layer(const xfeat_ctx* ctx, int i, const __half* x_split, 
   P.out_split = out_split; P.out_f32 = out_f32;
   const int max_tiles = cdiv(rows_cap, 128) * P.n_tiles;
   const int grid = max_tiles < ctx->sm_count ? max_tiles : ctx->sm_count;
-  if (NT == 128) {
-    XF_DYN_SMEM(mlp_gemm_kernel<128>, MlpCfg<128>::SMEM);
-    mlp_gemm_kernel<128><<<grid, ML_THREADS, MlpCfg<128>::SMEM, st>>>(P);
-  } else {
-    XF_DYN_SMEM(mlp_gemm_kernel<64>, MlpCfg<64>::SMEM);
-    mlp_gemm_kernel<64><<<grid, ML_THREADS, MlpCfg<64>::SMEM, st>>>(P);
-  }
+  XF_DYN_SMEM(mlp_gemm_kernel<NT>, MlpCfg<NT>::SMEM);
+  mlp_gemm_kernel<NT><<<grid, ML_THREADS, MlpCfg<NT>::SMEM, st>>>(P);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -228,10 +228,10 @@ size_t mnn_tc_workspace_bytes(int batch, int n1_max, int n2_max);
 int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                   int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
                   unsigned long long** best21, float** inv_s2, cudaStream_t st, int once, float abs_bound);
-// 0 = fp32 CUDA cores, 1 = tcgen05 split-fp16 with one GEMM per direction (default), 2 = tcgen05 single pass: one GEMM, the
+// 0 = fp32 CUDA cores, 1 = wgmma split-fp16 with one GEMM per direction (default), 2 = wgmma single pass: one GEMM, the
 // column arg-max by cross-lane reduction in the epilogue -- same results, but the epilogue then out-weighs the saved GEMM
 // (64 x 4096 x 4096: 0.75 ms vs 0.68 ms per call, tools/mnn_ab.py), so it is kept selectable, not default;
-// 3 = implementation 1 on CTA pairs (tcgen05 cta_group::2, M = 256 across two SMs, half the B tile per SM)
+// 3 = implementation 1 with one CTA per (row block, pair, direction) instead of the persistent kernel
 // 4 = filter + exact re-score (mnn_fast.cu): one fp16 pass per direction tracking top-1 / top-2, the three-term kernel only on
 // the rows whose gap is within the rounding bound -- same results as 1.  Measured (profiles/r02/mnn_probe.json, 64 x 4096^2):
 // the filter pass is bound by the ALU pipe (FMNMX at 16 lanes/clk: 370 us against 115 us of tensor time), and the descriptors of

@@ -12,14 +12,10 @@
 //           tie rule of the full kernel, scattered over the pass-1 result.
 // The result is identical to implementation 1 (the test-suite runs both), at ~1/3 of the tensor work.
 //
-// Pass-1 kernel: persistent CTAs (one per SM) over work items (pair, direction, 256-row block); warp 0 = TMA producer (A
-// slabs double buffered across items, 6-stage ring of 128-column B tiles, hi boxes only), warp 1 = MMA issuer
-// (2 slabs x 4 UMMA 128x128x16 per tile, accumulators double buffered in TMEM), warps 2-17 = epilogue: warp -> (TMEM lane
-// quarter, slab, 64-column half), one thread per row and half.  The epilogue is the bound (a 128x128x64 tile is 256 tensor
-// cycles) and a dependent chain per row, so it runs 4 warps per scheduler and is branch-light: per 16-column chunk a 3-input
-// max tree over two 8-column groups, a top-2 merge, and -- only when some lane's running maximum improves -- a predicated
-// save of the winning group's eight values; the column inside the group and the in-group runner-up are resolved once per
-// row at the end of the item, after the two column halves have been merged through shared memory.
+// Pass-1 kernel: persistent CTAs (one per SM) over work items (pair, direction, 256-row block); warp 8 = TMA producer (A
+// slabs double buffered across items, 6-stage ring of 128-column B tiles, hi boxes only), warps 0-7 = two consumer warpgroups,
+// one per 128-row slab: wgmma 64 x 128 x 16 into registers, then per row the maximum, its first column and the runner-up
+// value, reduced in-thread and across the four lanes of a row (mnn_tc.cu describes the fragment layout).
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -29,14 +25,8 @@ namespace xf {
 
 constexpr int MF_ROWS = 256, MF_BN = 128, MF_KP = 128, MF_BOX = 128 * 128;   // hi box: 128 rows x 64 halves
 constexpr int MF_NSB = 6;                                                      // B tile ring depth
-constexpr int MF_EPI_WARPS = 16, MF_THREADS = 64 + 32 * MF_EPI_WARPS;   // warp 0 TMA, warp 1 MMA, warps 2-17 epilogue
-constexpr size_t MF_SMEM = 1024 + (size_t)(4 + MF_NSB) * MF_BOX + 512 + 2 * 4 * 256 * sizeof(float);
-
-__device__ __forceinline__ float max3f(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
+constexpr int MF_THREADS = 288;                                              // warps 0-7: two consumer warpgroups, warp 8: TMA
+constexpr size_t MF_SMEM = 1024 + (size_t)(4 + MF_NSB) * MF_BOX + 512;
 
 // One warp per row: split row [hi(64) | lo(64)] (as split_kernel in mnn_tc.cu) plus the row's ||hi||, ||lo|| (in scaled
 // units) and the per-(pair) maxima of both over the set, as float bits (non-negative floats order like unsigned ints).
@@ -110,49 +100,6 @@ struct MfParams {
   __half *amb_rows0, *amb_rows1;      // compact operand rows per direction: (batch * n_pad) x 128 halves
 };
 
-// per-row running state of the filter pass
-struct MfRow {
-  float best, m2;     // maximum so far; largest value seen OUTSIDE the 8-column group that holds the maximum
-  float sin;          // runner-up INSIDE that group (== best when the maximum occurs twice in it)
-  int col;            // column of the maximum (first one inside its group)
-};
-
-// one 16-column chunk (two 8-column groups) of one row
-__device__ __forceinline__ void mf_process16(uint32_t (&r)[16], int cb, int n_cols, MfRow& st) {
-  if (cb + 16 > n_cols) {       // chunk straddles or lies past the last valid column (last tile only; warp-uniform)
-#pragma unroll
-    for (int j = 0; j < 16; ++j)
-      if (cb + j >= n_cols) r[j] = 0xff800000u;   // -inf
-  }
-  float g[2];
-#pragma unroll
-  for (int k = 0; k < 2; ++k)
-    g[k] = max3f(max3f(__uint_as_float(r[8 * k]), __uint_as_float(r[8 * k + 1]), __uint_as_float(r[8 * k + 2])),
-                 max3f(__uint_as_float(r[8 * k + 3]), __uint_as_float(r[8 * k + 4]), __uint_as_float(r[8 * k + 5])),
-                 fmaxf(__uint_as_float(r[8 * k + 6]), __uint_as_float(r[8 * k + 7])));
-  const float top = fmaxf(g[0], g[1]), sec = fminf(g[0], g[1]);
-  st.m2 = max3f(st.m2, sec, fminf(st.best, top));   // the old maximum (and its group) is "outside" once a new group takes over
-  const bool improve = top > st.best;               // strict: an equal value leaves m2 == best, i.e. an ambiguous row
-  if (__any_sync(0xffffffffu, improve)) {           // rare per lane (~ln N times per row), branch-free inside
-    const bool p0 = (g[0] == top);
-    float w[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) w[j] = p0 ? __uint_as_float(r[j]) : __uint_as_float(r[8 + j]);
-    int jj = 7, cnt = 0;
-#pragma unroll
-    for (int j = 7; j >= 0; --j) {
-      const bool eq = (w[j] == top);
-      jj = eq ? j : jj;
-      cnt += eq ? 1 : 0;
-      w[j] = eq ? -INFINITY : w[j];
-    }
-    const float others = max3f(max3f(w[0], w[1], w[2]), max3f(w[3], w[4], w[5]), fmaxf(w[6], w[7]));
-    st.sin = improve ? (cnt > 1 ? top : others) : st.sin;
-    st.col = improve ? cb + (p0 ? 0 : 8) + jj : st.col;
-  }
-  st.best = fmaxf(st.best, top);
-}
-
 __global__ void __launch_bounds__(MF_THREADS, 1) mnn_fast_kernel(const __grid_constant__ MfParams P) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -163,38 +110,25 @@ __global__ void __launch_bounds__(MF_THREADS, 1) mnn_fast_kernel(const __grid_co
   uint64_t* a_empty = bars + 2;                   // [2]
   uint64_t* b_full = bars + 4;                    // [MF_NSB]
   uint64_t* b_empty = b_full + MF_NSB;            // [MF_NSB]
-  uint64_t* acc_full = b_empty + MF_NSB;          // [2]
-  uint64_t* acc_empty = acc_full + 2;             // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* sMerge = reinterpret_cast<float*>(base + (4 + MF_NSB) * MF_BOX + 512);   // [item parity 2][field 4][256 rows]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int RB = P.n_pad / MF_ROWS;
   const int n_items = P.batch * 2 * RB;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(&P.m1);
     tc::tma_prefetch_desc(&P.m2);
     for (int i = 0; i < 2; ++i) {
       tc::mbar_init(&a_full[i], 1);
-      tc::mbar_init(&a_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], MF_EPI_WARPS);
+      tc::mbar_init(&a_empty[i], 8);
     }
     for (int i = 0; i < MF_NSB; ++i) {
       tc::mbar_init(&b_full[i], 1);
-      tc::mbar_init(&b_empty[i], 1);
+      tc::mbar_init(&b_empty[i], 8);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   // item -> (pair, dir, row block); every role walks the same sequence and skips the same (empty) items
   auto decode = [&](int item, int& pair, int& dir, int& row0, int& n_rows, int& n_cols) {
@@ -209,7 +143,7 @@ __global__ void __launch_bounds__(MF_THREADS, 1) mnn_fast_kernel(const __grid_co
     return row0 < n_rows && n_cols > 0;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (tc::elect_one()) {
       // ---------------- TMA producer ----------------
       uint32_t ai = 0, bi = 0;
@@ -236,111 +170,86 @@ __global__ void __launch_bounds__(MF_THREADS, 1) mnn_fast_kernel(const __grid_co
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      // ---------------- MMA issuer ----------------
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, MF_BN);
-      uint32_t ai = 0, bi = 0, tt = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int pair, dir, row0, n_rows, n_cols;
-        if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
-        const int T = (n_cols + MF_BN - 1) / MF_BN;
-        const int ab = ai & 1;
-        tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
-        const uint64_t da0 = tc::make_desc_sw128(tc::smem_u32(sA + (ab * 2 + 0) * MF_BOX), 1024);
-        const uint64_t da1 = tc::make_desc_sw128(tc::smem_u32(sA + (ab * 2 + 1) * MF_BOX), 1024);
-        for (int t = 0; t < T; ++t, ++bi, ++tt) {
-          const int s = bi % MF_NSB, as = tt & 1;
-          tc::mbar_wait(&b_full[s], (bi / MF_NSB) & 1);
-          tc::mbar_wait(&acc_empty[as], ((tt >> 1) & 1) ^ 1);
-          tc::tc_fence_after();
-          const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + s * MF_BOX), 1024);
-          const uint32_t d = tmem + as * 256;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_f16(d, da0 + 2 * k, db + 2 * k, idesc, k ? 1u : 0u);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_f16(d + 128, da1 + 2 * k, db + 2 * k, idesc, k ? 1u : 0u);
-          tc::umma_commit(&b_empty[s]);
-          tc::umma_commit(&acc_full[as]);
-        }
-        tc::umma_commit(&a_empty[ab]);     // the A slabs may be overwritten once every MMA of this item has completed
-        ++ai;
-      }
-    }
-    __syncwarp();
   } else {
-    // ---------------- epilogue: 16 warps = (TMEM lane quarter q) x (slab) x (64-column half hc) ----------------
-    // The reduction is a dependent chain per row, so thread-level parallelism (4 warps per scheduler) is what fills the
-    // issue slots; each warp drains 4 x 16 columns of one slab per tile.
-    const int e = warp - 2;
-    const int q = warp & 3, slab = (e >> 2) & 1, hc = e >> 3;
-    const int rl = slab * 128 + q * 32 + lane;                 // row of the item owned by this thread
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16) + slab * 128 + hc * 64;
-    uint32_t tt = 0, icount = 0;
+    // ---------------- consumer warpgroup `slab`: hi.hi^T tile + per-row top-1 (value, first column) and top-2 value ----------------
+    const int slab = warp >> 2, wt = threadIdx.x & 127;
+    const int cq = 2 * (lane & 3);
+    constexpr uint32_t HALF = (64 * 128) >> 4;
+    float acc0[64], acc1[64];
+    uint32_t ai = 0, bi = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       int pair, dir, row0, n_rows, n_cols;
       if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
       const int T = (n_cols + MF_BN - 1) / MF_BN;
-      const int row = row0 + rl;
-      MfRow st;
-      st.best = -INFINITY; st.m2 = -INFINITY; st.sin = -INFINITY; st.col = 0;
-
-      for (int t = 0; t < T; ++t, ++tt) {
-        const int as = tt & 1;
-        tc::mbar_wait(&acc_full[as], (tt >> 1) & 1);
-        tc::tc_fence_after();
-        const uint32_t tb = lane_addr + as * 256;
-        const int cb = t * MF_BN + hc * 64;
-        // all four loads first, ONE wait, and the TMEM buffer goes straight back to the MMA warp: the accumulator double buffer
-        // then hides the whole reduction (holding the buffer across the reduction made the tile time MMA + epilogue / 2)
-        uint32_t ra[16], rb[16], rc[16], rd[16];
-        __syncwarp();
-        tc::tmem_ld_32x16(tb, ra);
-        tc::tmem_ld_32x16(tb + 16, rb);
-        tc::tmem_ld_32x16(tb + 32, rc);
-        tc::tmem_ld_32x16(tb + 48, rd);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&acc_empty[as]);   // all TMEM reads of this buffer (by this warp) are done
-        mf_process16(ra, cb, n_cols, st);
-        mf_process16(rb, cb + 16, n_cols, st);
-        mf_process16(rc, cb + 32, n_cols, st);
-        mf_process16(rd, cb + 48, n_cols, st);
-      }
-
-      // ---- end of the item: merge the two column halves of every row through shared memory (double buffered by item) ----
-      float* mg = sMerge + (icount & 1) * (4 * 256);
-      ++icount;
-      if (hc == 1) {
-        mg[0 * 256 + rl] = st.best;
-        mg[1 * 256 + rl] = st.m2;
-        mg[2 * 256 + rl] = st.sin;
-        mg[3 * 256 + rl] = __int_as_float(st.col);
-      }
-      asm volatile("bar.sync 1, 512;" ::: "memory");     // epilogue warps only
-      if (hc == 0) {
-        const float ob = mg[0 * 256 + rl], om2 = mg[1 * 256 + rl];
-        const bool other = ob > st.best;                  // a tie keeps the lower columns; the row is ambiguous anyway
-        st.m2 = max3f(st.m2, om2, fminf(st.best, ob));
-        if (other) {
-          st.best = ob;
-          st.sin = mg[2 * 256 + rl];
-          st.col = __float_as_int(mg[3 * 256 + rl]);
+      const int ab = ai & 1;
+      tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
+      const uint64_t da = tc::make_desc_sw128(tc::smem_u32(sA + (ab * 2 + slab) * MF_BOX), 1024);
+      float best[4], sec[4];
+      int col[4];
+#pragma unroll
+      for (int h = 0; h < 4; ++h) { best[h] = -INFINITY; sec[h] = -INFINITY; col[h] = 0; }
+      for (int t = 0; t < T; ++t, ++bi) {
+        const int s = bi % MF_NSB;
+        tc::mbar_wait(&b_full[s], (bi / MF_NSB) & 1);
+        const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + s * MF_BOX), 1024);
+        tc::wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          tc::wgmma_f16<128>(acc0, da + 2 * k, db + 2 * k, k ? 1u : 0u);
+          tc::wgmma_f16<128>(acc1, da + HALF + 2 * k, db + 2 * k, k ? 1u : 0u);
         }
-        const float second = fmaxf(st.m2, st.sin);
-        const bool live = row < n_rows;
+        tc::wgmma_commit();
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) {
+          tc::mbar_arrive(&b_empty[s]);
+          if (t == T - 1) tc::mbar_arrive(&a_empty[ab]);
+        }
+        const int cb = t * MF_BN, nv = n_cols - cb;
+#pragma unroll
+        for (int h = 0; h < 4; ++h)
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = 8 * j + cq + e;
+              const float v = (c < nv) ? tc::frag_val(acc0, acc1, h, j, e) : -INFINITY;
+              // columns ascending: a strictly larger value takes over (the old maximum becomes the runner-up), an equal one
+              // leaves the first column and makes the runner-up equal to the maximum (an ambiguous row)
+              sec[h] = fmaxf(sec[h], fminf(v, best[h]));
+              if (v > best[h]) { best[h] = v; col[h] = cb + c; }
+            }
+      }
+      ++ai;
+      // merge the four lanes of every row: exact top-1 (lowest column on ties) and top-2 of the union
+#pragma unroll
+      for (int h = 0; h < 4; ++h)
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float ob = __shfl_xor_sync(0xffffffffu, best[h], o), os = __shfl_xor_sync(0xffffffffu, sec[h], o);
+          const int oc = __shfl_xor_sync(0xffffffffu, col[h], o);
+          const float nsec = fmaxf(fmaxf(sec[h], os), fminf(best[h], ob));
+          if (ob > best[h] || (ob == best[h] && oc < col[h])) { best[h] = ob; col[h] = oc; }
+          sec[h] = nsec;
+        }
+      const float2* norms = dir ? P.norms2 : P.norms1;
+      const unsigned* mo = (dir ? P.maxn1 : P.maxn2) + pair * 2;            // the OTHER set's maxima
+      const float Hmax = __uint_as_float(__ldg(mo)), Lmax = __uint_as_float(__ldg(mo + 1));
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {
+        const int row = row0 + slab * 128 + tc::frag_row(wt, h);
+        const bool live = (lane & 3) == 0 && row < n_rows;
         bool amb = false;
         if (live) {
-          const float2 nr = __ldg((dir ? P.norms2 : P.norms1) + (int64_t)pair * P.n_pad + row);
-          const unsigned* mo = (dir ? P.maxn1 : P.maxn2) + pair * 2;            // the OTHER set's maxima
-          const float Hmax = __uint_as_float(__ldg(mo)), Lmax = __uint_as_float(__ldg(mo + 1));
+          const float2 nr = __ldg(norms + (int64_t)pair * P.n_pad + row);
           // |S~ - S| <= ||hi_i|| Lmax + ||lo_i|| Hmax for every column; both the best and a competitor may be off by that much;
           // 2^-14 ||hi_i|| Hmax covers the fp32 accumulation-order difference between the one-term and the three-term sums.
           const float tau = 2.1f * (nr.x * Lmax + nr.y * Hmax) + 6.2e-5f * nr.x * Hmax;
-          amb = !(st.best - second > tau);                                       // also true for NaN / -inf oddities
+          amb = !(best[h] - sec[h] > tau);                                      // also true for NaN / -inf oddities
           unsigned long long* out = dir ? P.best21 : P.best12;
-          out[(int64_t)pair * (dir ? P.n2_max : P.n1_max) + row] = pack_vi(st.best, (uint32_t)st.col);
+          out[(int64_t)pair * (dir ? P.n2_max : P.n1_max) + row] = pack_vi(best[h], (uint32_t)col[h]);
         }
         // ambiguous rows: append (row index + split operand row) to the compact list of this (pair, direction)
         unsigned mask = __ballot_sync(0xffffffffu, amb);
@@ -363,12 +272,6 @@ __global__ void __launch_bounds__(MF_THREADS, 1) mnn_fast_kernel(const __grid_co
         }
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 512);
   }
 }
 

@@ -1,20 +1,15 @@
-// Mutual-NN similarity scan on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), fp32-equivalent precision.
+// Mutual-NN similarity scan on the Hopper tensor cores (wgmma + TMA), fp32-equivalent precision.
 //
 // fp32-equivalent via operand splitting: x*s = hi + lo with hi, lo in fp16 (s = power of two chosen from max|x| so that
 // hi uses the fp16 range and lo stays normal), rows stored as [hi(64) | lo(64)] halves, and three K = 64 fp16 GEMM blocks
-// with fp32 accumulation into the same TMEM tile
+// with fp32 accumulation into the same register tile
 //      S = hi1.hi2^T + hi1.lo2^T + lo1.hi2^T
-// (the dropped lo.lo term is ~2^-22 relative, below fp32 accumulation noise).  The blocks are selected by the UMMA
+// (the dropped lo.lo term is ~2^-22 relative, below fp32 accumulation noise).  The blocks are selected by the wgmma
 // descriptor addresses (hi box / lo box of each operand), so nothing is stored twice.  The same two arrays serve both scan
-// directions (rows of F1 against F2, rows of F2 against F1), which add the same three products in the same order:
-// S12[i][j] and S21[j][i] are bit-identical.
+// directions (rows of F1 against F2, rows of F2 against F1), which add the same three products in the same order.
 //
-// One CTA = 256 rows (two M=128 accumulator slabs) x all 128-column tiles of the other set:
-//   warp 0   : TMA producer (A slabs once, then the B tile ring, 128B-swizzled K-major boxes of 64 halves x 128 rows)
-//   warp 1   : TMEM allocation + single-thread tcgen05.mma issue (2 slabs x 3 K-blocks x 4 UMMA 128x128x16 per tile)
-//   warps 2-5: epilogue, one TMEM lane quarter each: tcgen05.ld 32 columns at a time, running row arg-max in registers
-// The accumulators are double buffered in TMEM (2 x 256 columns), so the arg-max of tile t overlaps the MMAs of t+1.
-// Nothing but the final (value, index) per row ever leaves the SM.
+// One work item = 256 rows (two 128-row slabs) x all 128-column tiles of the other set; TMA streams the B tiles through a
+// ring of stages while the two consumer warpgroups reduce.  Nothing but the final (value, index) per row ever leaves the SM.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -35,10 +30,7 @@ PFN_encodeTiled get_encode_tiled() {
 }
 
 constexpr int TC_ROWS = 256, TC_BN = 128, TC_KP = 128, TC_BOX_BYTES = 128 * 128;  // operand row [hi(64) | lo(64)]; box = 128 rows x 128 B
-constexpr int TC_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2-9 epilogue (two per TMEM lane quarter)
-constexpr size_t TC_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256 + 2 * 128 * 8;
-constexpr int TC1_EPI_WARPS = 16, TC1_THREADS = 64 + 32 * TC1_EPI_WARPS;   // single-pass variant: warps 2-17 epilogue
-constexpr size_t TC1_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256 + 3 * 2 * 128 * 8 + 2 * 2 * 4 * 128 * 4 + TC1_EPI_WARPS * 64 * 4;
+constexpr size_t TC_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256;
 
 __global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ f, const int* __restrict__ np, int n_max,
                                                      int64_t stride, unsigned* __restrict__ out) {
@@ -91,9 +83,66 @@ struct TcMaps4 {
   CUtensorMap a0, b0, a1, b1;
 };
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Hopper mapping (shared by the kernels below): 256 rows per work item = two 128-row slabs, one consumer warpgroup per slab
+// (warps 0-3 / 4-7) issuing wgmma 64 x 128 x 16 for its two 64-row halves into registers; warp 8 = TMA producer.  A thread
+// holds, per tile, rows 16w + l/4 + {0, 8, 64, 72} of its slab (w = warp in the group, l = lane) and columns 8j + 2(l%4) + {0,1}.
+// The row arg-max is reduced in-thread, then across the four lanes of a row as packed (value, ~column) 64-bit maxima
+// (pack_vi: larger value, then lower column -- torch's first-index rule).
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int MT_THREADS = 288;           // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr uint32_t MT_HALF = (64 * 128) >> 4;   // descriptor offset of rows 64-127 of a slab
+
+// three-term S tile of one slab: hi.hi + (dir ? lo.hi, hi.lo : hi.lo, lo.hi), both directions in the same order so that
+// S12[i][j] and S21[j][i] come out of the same three products
+__device__ __forceinline__ void mnn_tile_mma(float (&acc0)[64], float (&acc1)[64], uint32_t a_slab, uint32_t b_stage, int dir) {
+  const int a_sel[3] = {0, dir ? 1 : 0, dir ? 0 : 1};
+  const int b_sel[3] = {0, dir ? 0 : 1, dir ? 1 : 0};
+  tc::wgmma_fence();
+#pragma unroll
+  for (int kb = 0; kb < 3; ++kb) {
+    const uint64_t da = tc::make_desc_sw128(a_slab + a_sel[kb] * TC_BOX_BYTES, 1024);
+    const uint64_t db = tc::make_desc_sw128(b_stage + b_sel[kb] * TC_BOX_BYTES, 1024);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {   // 16 halves = 32 B = 2 x 16-byte units along K inside the 128 B swizzle row
+      tc::wgmma_f16<128>(acc0, da + 2 * k, db + 2 * k, (kb | k) ? 1u : 0u);
+      tc::wgmma_f16<128>(acc1, da + MT_HALF + 2 * k, db + 2 * k, (kb | k) ? 1u : 0u);
+    }
+  }
+  tc::wgmma_commit();
+  tc::wgmma_wait<0>();
+  tc::acc_fence(acc0);
+  tc::acc_fence(acc1);
+}
+
+// running row arg-max of the thread's four rows over one tile (columns col0 .. col0+127, the first n_valid of them real)
+__device__ __forceinline__ void mnn_row_argmax(const float (&acc0)[64], const float (&acc1)[64], int col0, int n_valid,
+                                               int lane, unsigned long long (&best)[4]) {
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    float m = -INFINITY;
+    int c = -1;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float v = tc::frag_val(acc0, acc1, h, j, e);
+        const int cc = 8 * j + cq + e;
+        if (cc < n_valid && v > m) { m = v; c = cc; }   // strict, columns ascending: first index wins ties
+      }
+    unsigned long long p = (c >= 0) ? pack_vi(m, (uint32_t)(col0 + c)) : 0ull;
+    unsigned long long o = __shfl_xor_sync(0xffffffffu, p, 1);
+    p = o > p ? o : p;
+    o = __shfl_xor_sync(0xffffffffu, p, 2);
+    p = o > p ? o : p;
+    best[h] = p > best[h] ? p : best[h];
+  }
+}
+
 // rows_cnt (optional): [pair][dir] number of rows of the A array to scan (the compact lists of mnn_fast.cu) instead of the
 // set size; row_map (optional): [pair][dir][n_pad] output row of compact row r.
-__global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_kernel(const __grid_constant__ TcMaps4 maps,
+__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_kernel(const __grid_constant__ TcMaps4 maps,
                                                                const int* __restrict__ n1p, int n1_max,
                                                                const int* __restrict__ n2p, int n2_max, int n_pad,
                                                                unsigned long long* __restrict__ best12,
@@ -119,37 +168,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_kernel(const __grid_cons
   uint64_t* a_full = bars;
   uint64_t* b_full = bars + 1;     // [2]
   uint64_t* b_empty = bars + 3;    // [2]
-  uint64_t* acc_full = bars + 5;   // [2]
-  uint64_t* acc_empty = bars + 7;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  unsigned long long* sMerge = reinterpret_cast<unsigned long long*>(bars + 12);   // [2 slabs][128 rows]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int T = (n_cols + TC_BN - 1) / TC_BN;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(mapA);
     tc::tma_prefetch_desc(mapB);
     tc::mbar_init(a_full, 1);
     for (int i = 0; i < 2; ++i) {
       tc::mbar_init(&b_full[i], 1);
-      tc::mbar_init(&b_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 8);
+      tc::mbar_init(&b_empty[i], 8);   // one arrival per consumer warp
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    if (T > 0 && tc::elect_one()) {   // no column tiles: nothing may be left in flight when the CTA exits
+  if (warp == 8) {
+    if (T > 0 && tc::elect_one()) {
       // ---------------- TMA producer ----------------
       const int arow = pair * n_pad + row0;
       tc::mbar_expect_tx(a_full, 4 * TC_BOX_BYTES);
@@ -166,136 +202,44 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_kernel(const __grid_cons
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      // ---------------- MMA issuer ----------------
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, TC_BN);
-      // K-blocks of x.y = hi.hi + hi.lo + lo.hi, taken from the [hi | lo] boxes of the two operands.  Direction 1 (A = F2,
-      // B = F1) swaps the roles of the last two blocks so both directions add the same three products in the same order and
-      // S12[i][j] == S21[j][i] bit for bit.
-      const int a_sel[3] = {0, dir ? 1 : 0, dir ? 0 : 1};
-      const int b_sel[3] = {0, dir ? 0 : 1, dir ? 1 : 0};
-      if (T > 0) tc::mbar_wait(a_full, 0);   // (nothing was loaded when there are no column tiles)
-      for (int t = 0; t < T; ++t) {
-        const int s = t & 1, ph = (t >> 1) & 1;
-        tc::mbar_wait(&b_full[s], ph);
-        tc::mbar_wait(&acc_empty[s], ph ^ 1);
-        tc::tc_fence_after();
-#pragma unroll
-        for (int slab = 0; slab < 2; ++slab) {
-          const uint32_t d = tmem + s * 256 + slab * 128;
-#pragma unroll
-          for (int kb = 0; kb < 3; ++kb) {
-            const uint64_t da = tc::make_desc_sw128(tc::smem_u32(sA + (slab * 2 + a_sel[kb]) * TC_BOX_BYTES), 1024);
-            const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + (s * 2 + b_sel[kb]) * TC_BOX_BYTES), 1024);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)  // 16 halves = 32 B = 2 x 16-byte units along K inside the 128 B swizzle row
-              tc::umma_f16(d, da + 2 * k, db + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-        }
-        tc::umma_commit(&b_empty[s]);    // B stage may be refilled once these MMAs have read it
-        tc::umma_commit(&acc_full[s]);   // accumulators of tile t are complete
-      }
-    }
-    __syncwarp();
   } else {
-    // ---------------- epilogue: running row arg-max ----------------
-    // warps 2-9: TMEM lane quarter q = warp & 3 (hardware rule: a warp reaches lanes 32*(warp%4)..+31), column half
-    // hc = (warp - 2) >> 2 of each 128-column slab.  tcgen05.ld of chunk c+1 is in flight while chunk c is reduced.
-    const int q = warp & 3, hc = (warp - 2) >> 2;
-    float best[2] = {-INFINITY, -INFINITY};
-    uint32_t bidx[2] = {0xffffffffu, 0xffffffffu};
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-    auto reduce_chunk = [&](const uint32_t (&r)[32], int col0, int slab) {
-      if (col0 + 32 <= n_cols) {
-        float m = __uint_as_float(r[0]);
-#pragma unroll
-        for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(r[j]));
-        if (m > best[slab]) {            // strict: earlier columns win ties (torch.max / argmax rule)
-          int j0 = 31;
-#pragma unroll
-          for (int j = 30; j >= 0; --j)
-            if (__uint_as_float(r[j]) == m) j0 = j;
-          best[slab] = m;
-          bidx[slab] = (uint32_t)(col0 + j0);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float v = __uint_as_float(r[j]);
-          if (col0 + j < n_cols && v > best[slab]) { best[slab] = v; bidx[slab] = (uint32_t)(col0 + j); }
-        }
-      }
-    };
+    // ---------------- consumer warpgroup `slab`: wgmma + running row arg-max ----------------
+    const int slab = warp >> 2, wt = threadIdx.x & 127;
+    float acc0[64], acc1[64];
+    unsigned long long best[4] = {0ull, 0ull, 0ull, 0ull};
+    if (T > 0) tc::mbar_wait(a_full, 0);
+    const uint32_t a_slab = tc::smem_u32(sA + slab * 2 * TC_BOX_BYTES);
     for (int t = 0; t < T; ++t) {
-      const int s = t & 1, ph = (t >> 1) & 1;
-      tc::mbar_wait(&acc_full[s], ph);
-      tc::tc_fence_after();
-      // this warp's 4 chunks of the tile: (slab 0, cols hc*64 + {0,32}), (slab 1, cols hc*64 + {0,32})
-      uint32_t ra[32], rb[32];
-      const uint32_t tb = lane_addr + s * 256 + hc * 64;
-      const int cb = t * TC_BN + hc * 64;
+      const int s = t & 1;
+      tc::mbar_wait(&b_full[s], (t >> 1) & 1);
+      mnn_tile_mma(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), dir);
       __syncwarp();
-      tc::tmem_ld_32x32(tb, ra);
-      tc::tmem_ld_wait();
-      __syncwarp();
-      tc::tmem_ld_32x32(tb + 32, rb);
-      reduce_chunk(ra, cb, 0);
-      tc::tmem_ld_wait();
-      __syncwarp();
-      tc::tmem_ld_32x32(tb + 128, ra);
-      reduce_chunk(rb, cb + 32, 0);
-      tc::tmem_ld_wait();
-      __syncwarp();
-      tc::tmem_ld_32x32(tb + 128 + 32, rb);
-      reduce_chunk(ra, cb, 1);
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[s]);   // all TMEM reads of this buffer are done
-      reduce_chunk(rb, cb + 32, 1);
+      if (lane == 0) tc::mbar_arrive(&b_empty[s]);   // this warp's reads of the B stage are complete
+      mnn_row_argmax(acc0, acc1, t * TC_BN, n_cols - t * TC_BN, lane, best);
     }
-    // merge the two column halves of every row (lower column index wins ties through the packed compare)
-    unsigned long long pk[2];
+    if ((lane & 3) == 0) {
 #pragma unroll
-    for (int slab = 0; slab < 2; ++slab) pk[slab] = (bidx[slab] == 0xffffffffu) ? 0ull : pack_vi(best[slab], bidx[slab]);
-    if (hc == 1) {
-      sMerge[0 * 128 + q * 32 + lane] = pk[0];
-      sMerge[1 * 128 + q * 32 + lane] = pk[1];
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");     // epilogue warps only
-    if (hc == 0) {
-#pragma unroll
-      for (int slab = 0; slab < 2; ++slab) {
-        const unsigned long long o = sMerge[slab * 128 + q * 32 + lane];
-        const unsigned long long m = o > pk[slab] ? o : pk[slab];
-        const int row = row0 + slab * 128 + q * 32 + lane;
+      for (int h = 0; h < 4; ++h) {
+        const int row = row0 + slab * 128 + tc::frag_row(wt, h);
         if (row < n_rows) {
           const int orow = row_map ? __ldg(row_map + (int64_t)(pair * 2 + dir) * n_pad + row) : row;
-          out[(int64_t)pair * out_stride + orow] = m;
+          out[(int64_t)pair * out_stride + orow] = best[h];
         }
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 512);
   }
 }
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Persistent form of mnn_tc_kernel (round 2): one CTA per SM walks work items (pair, direction, 256-row block) instead of one
-// CTA per item, so barrier initialisation, the TMEM allocation and -- above all -- the 64 KB A-slab load of the NEXT item overlap
-// the tiles of the current one (A slabs double buffered, 2-stage ring of B tiles).  13.8 waves of one-shot CTAs paid the
-// prologue and the drain 14 times; here they are paid once.  Same arithmetic, same epilogue, same results.
+// Persistent form of mnn_tc_kernel: one CTA per SM walks work items (pair, direction, 256-row block) instead of one CTA per
+// item, so barrier initialisation and -- above all -- the 64 KB A-slab load of the NEXT item overlap the tiles of the current
+// one (A slabs double buffered, 3-stage ring of B tiles).  Same arithmetic, same results.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int TCP_NSB = 2;   // (three stages would need 232.7 KB: 256 bytes over the per-CTA maximum)
-constexpr size_t TCP_SMEM = 1024 + (size_t)(8 + 2 * TCP_NSB) * TC_BOX_BYTES + 256 + 2 * 128 * 8;
+constexpr int TCP_NSB = 3;
+constexpr size_t TCP_SMEM = 1024 + (size_t)(8 + 2 * TCP_NSB) * TC_BOX_BYTES + 256;
 
-__global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
+__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
                                                                        const int* __restrict__ n1p, int n1_max,
                                                                        const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
                                                                        unsigned long long* __restrict__ best12,
@@ -309,38 +253,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_persist_kernel(const __g
   uint64_t* a_empty = bars + 2;                   // [2]
   uint64_t* b_full = bars + 4;                    // [TCP_NSB]
   uint64_t* b_empty = b_full + TCP_NSB;           // [TCP_NSB]
-  uint64_t* acc_full = b_empty + TCP_NSB;         // [2]
-  uint64_t* acc_empty = acc_full + 2;             // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  unsigned long long* sMerge = reinterpret_cast<unsigned long long*>(base + (8 + 2 * TCP_NSB) * TC_BOX_BYTES + 256);   // [2 slabs][128 rows]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int RB = n_pad / TC_ROWS;
   const int n_items = batch * 2 * RB;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(&maps.m1);
     tc::tma_prefetch_desc(&maps.m2);
     for (int i = 0; i < 2; ++i) {
       tc::mbar_init(&a_full[i], 1);
-      tc::mbar_init(&a_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 8);
+      tc::mbar_init(&a_empty[i], 8);
     }
     for (int i = 0; i < TCP_NSB; ++i) {
       tc::mbar_init(&b_full[i], 1);
-      tc::mbar_init(&b_empty[i], 1);
+      tc::mbar_init(&b_empty[i], 8);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   // item -> (pair, dir, row block); every role walks the same sequence and skips the same (empty) items
   auto decode = [&](int item, int& pair, int& dir, int& row0, int& n_rows, int& n_cols) {
@@ -355,7 +286,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_persist_kernel(const __g
     return row0 < n_rows && n_cols > 0;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (tc::elect_one()) {
       uint32_t ai = 0, bi = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -383,159 +314,53 @@ __global__ void __launch_bounds__(TC_THREADS, 1) mnn_tc_persist_kernel(const __g
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, TC_BN);
-      uint32_t ai = 0, bi = 0, tt = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int pair, dir, row0, n_rows, n_cols;
-        if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
-        const int T = (n_cols + TC_BN - 1) / TC_BN;
-        const int ab = ai & 1;
-        // K-block order hi.hi, then (dir ? lo.hi, hi.lo : hi.lo, lo.hi): S12[i][j] == S21[j][i] bit for bit (see mnn_tc_kernel)
-        const int a_sel[3] = {0, dir ? 1 : 0, dir ? 0 : 1};
-        const int b_sel[3] = {0, dir ? 0 : 1, dir ? 1 : 0};
-        tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
-        for (int t = 0; t < T; ++t, ++bi, ++tt) {
-          const int s = bi % TCP_NSB, as = tt & 1;
-          tc::mbar_wait(&b_full[s], (bi / TCP_NSB) & 1);
-          tc::mbar_wait(&acc_empty[as], ((tt >> 1) & 1) ^ 1);
-          tc::tc_fence_after();
-#pragma unroll
-          for (int slab = 0; slab < 2; ++slab) {
-            const uint32_t d = tmem + as * 256 + slab * 128;
-#pragma unroll
-            for (int kb = 0; kb < 3; ++kb) {
-              const uint64_t da = tc::make_desc_sw128(tc::smem_u32(sA + ((ab * 2 + slab) * 2 + a_sel[kb]) * TC_BOX_BYTES), 1024);
-              const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + (s * 2 + b_sel[kb]) * TC_BOX_BYTES), 1024);
-#pragma unroll
-              for (int k = 0; k < 4; ++k) tc::umma_f16(d, da + 2 * k, db + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            }
-          }
-          tc::umma_commit(&b_empty[s]);
-          tc::umma_commit(&acc_full[as]);
-        }
-        tc::umma_commit(&a_empty[ab]);
-        ++ai;
-      }
-    }
-    __syncwarp();
   } else {
-    // epilogue: as mnn_tc_kernel (TMEM lane quarter q, column half hc), state reset per item
-    const int q = warp & 3, hc = (warp - 2) >> 2;
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-    uint32_t tt = 0;
+    const int slab = warp >> 2, wt = threadIdx.x & 127;
+    float acc0[64], acc1[64];
+    uint32_t ai = 0, bi = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
       int pair, dir, row0, n_rows, n_cols;
       if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
       const int T = (n_cols + TC_BN - 1) / TC_BN;
-      float best[2] = {-INFINITY, -INFINITY};
-      uint32_t bidx[2] = {0xffffffffu, 0xffffffffu};
-      auto reduce_chunk = [&](const uint32_t (&r)[32], int col0, int slab) {
-        if (col0 + 32 <= n_cols) {
-          float m = __uint_as_float(r[0]);
-#pragma unroll
-          for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(r[j]));
-          if (m > best[slab]) {            // strict: earlier columns win ties (torch.max / argmax rule)
-            int j0 = 31;
-#pragma unroll
-            for (int j = 30; j >= 0; --j)
-              if (__uint_as_float(r[j]) == m) j0 = j;
-            best[slab] = m;
-            bidx[slab] = (uint32_t)(col0 + j0);
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float v = __uint_as_float(r[j]);
-            if (col0 + j < n_cols && v > best[slab]) { best[slab] = v; bidx[slab] = (uint32_t)(col0 + j); }
-          }
+      const int ab = ai & 1;
+      tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
+      const uint32_t a_slab = tc::smem_u32(sA + (ab * 2 + slab) * 2 * TC_BOX_BYTES);
+      unsigned long long best[4] = {0ull, 0ull, 0ull, 0ull};
+      for (int t = 0; t < T; ++t, ++bi) {
+        const int s = bi % TCP_NSB;
+        tc::mbar_wait(&b_full[s], (bi / TCP_NSB) & 1);
+        mnn_tile_mma(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), dir);
+        __syncwarp();
+        if (lane == 0) {
+          tc::mbar_arrive(&b_empty[s]);
+          if (t == T - 1) tc::mbar_arrive(&a_empty[ab]);   // the A slabs may be overwritten
         }
-      };
-      for (int t = 0; t < T; ++t, ++tt) {
-        const int as = tt & 1;
-        tc::mbar_wait(&acc_full[as], (tt >> 1) & 1);
-        tc::tc_fence_after();
-        uint32_t ra[32], rb[32];
-        const uint32_t tb = lane_addr + as * 256 + hc * 64;
-        const int cb = t * TC_BN + hc * 64;
-        __syncwarp();
-        tc::tmem_ld_32x32(tb, ra);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 32, rb);
-        reduce_chunk(ra, cb, 0);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 128, ra);
-        reduce_chunk(rb, cb + 32, 0);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 128 + 32, rb);
-        reduce_chunk(ra, cb, 1);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&acc_empty[as]);
-        reduce_chunk(rb, cb + 32, 1);
+        mnn_row_argmax(acc0, acc1, t * TC_BN, n_cols - t * TC_BN, lane, best);
       }
-      // merge the two column halves of every row (lower column index wins ties through the packed compare)
-      unsigned long long pk[2];
-#pragma unroll
-      for (int slab = 0; slab < 2; ++slab) pk[slab] = (bidx[slab] == 0xffffffffu) ? 0ull : pack_vi(best[slab], bidx[slab]);
-      asm volatile("bar.sync 1, 256;" ::: "memory");     // the previous item's merge reads are complete
-      if (hc == 1) {
-        sMerge[0 * 128 + q * 32 + lane] = pk[0];
-        sMerge[1 * 128 + q * 32 + lane] = pk[1];
-      }
-      asm volatile("bar.sync 1, 256;" ::: "memory");     // epilogue warps only
-      if (hc == 0) {
+      ++ai;
+      if ((lane & 3) == 0) {
         unsigned long long* out = dir ? best21 : best12;
         const int out_stride = dir ? n2_max : n1_max;
 #pragma unroll
-        for (int slab = 0; slab < 2; ++slab) {
-          const unsigned long long o = sMerge[slab * 128 + q * 32 + lane];
-          const unsigned long long m = o > pk[slab] ? o : pk[slab];
-          const int row = row0 + slab * 128 + q * 32 + lane;
-          if (row < n_rows) out[(int64_t)pair * out_stride + row] = m;
+        for (int h = 0; h < 4; ++h) {
+          const int row = row0 + slab * 128 + tc::frag_row(wt, h);
+          if (row < n_rows) out[(int64_t)pair * out_stride + row] = best[h];
         }
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 512);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Single-pass variant (default): S is computed ONCE; the same accumulator tile yields the running row arg-max (as above) and
-// the column arg-max.  A thread owns a row, so a column maximum is a reduction across the 32 lanes of a warp:
-//   1. the two slabs are merged in-thread, then a transposing butterfly (31 shuffles per 32x32 chunk; lane l ends with the
-//      maximum of column l over the warp's 64 rows);
-//   2. the 32 maxima go through shared memory back to every lane (one store, 8 broadcast 128-bit loads), and each lane
-//      tests its own values for equality with them; the attaining rows race with atomicMin on the row index, which is
-//      torch's first-index rule;
-//   3. after a per-tile barrier one thread per column merges the CTA's four row groups and issues one 64-bit atomicMax of
-//      (value, ~row) per column: the same packed format mnn_tc_kernel's second GEMM produced, so mnn_finalize_kernel is
-//      unchanged and the result is identical.
-// Halves the tensor-pipe work of mnn_tc_kernel, which ncu shows is the bound (80 % pipe-active, profiles/r01).
-__device__ __forceinline__ void col_butterfly(float (&a)[32], int lane) {
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    const bool up = (lane & o) != 0;
-#pragma unroll
-    for (int j = 0; j < o; ++j) {
-      const float keep = up ? a[j + o] : a[j];
-      const float send = up ? a[j] : a[j + o];
-      a[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, o));
-    }
-  }
-}
+// Single-pass variant (xfeat_set_mnn_impl(2)): S is computed ONCE; the same accumulator tile yields the running row arg-max
+// (as above) and the column arg-max: per column, the thread's best of its four rows (rows ascending: first index wins), a
+// packed (value, ~row) maximum across the eight row lanes of the warp (shuffles), across the CTA's eight warps in shared memory
+// (64-bit atomicMax), then one global 64-bit atomicMax per column and tile -- the packed format mnn_tc_kernel's second
+// direction produces, so mnn_finalize_kernel is unchanged and the result is identical.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr size_t TC1_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256 + 2 * 128 * 8;
 
-__global__ void __launch_bounds__(TC1_THREADS, 1) mnn_tc_once_kernel(const __grid_constant__ TcMaps maps,
+__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_once_kernel(const __grid_constant__ TcMaps maps,
                                                                     const int* __restrict__ n1p, int n1_max,
                                                                     const int* __restrict__ n2p, int n2_max, int n_pad,
                                                                     unsigned long long* __restrict__ best12,
@@ -554,41 +379,26 @@ __global__ void __launch_bounds__(TC1_THREADS, 1) mnn_tc_once_kernel(const __gri
   uint64_t* a_full = bars;
   uint64_t* b_full = bars + 1;     // [2]
   uint64_t* b_empty = bars + 3;    // [2]
-  uint64_t* acc_full = bars + 5;   // [2]
-  uint64_t* acc_empty = bars + 7;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  unsigned long long* sMerge = reinterpret_cast<unsigned long long*>(bars + 12);   // [3 column quarters][2 slabs][128 rows]
-  float* sVal = reinterpret_cast<float*>(sMerge + 3 * 256);                         // [2 tile parities][4 row groups][128 columns]
-  unsigned* sRow = reinterpret_cast<unsigned*>(sVal + 2 * 4 * 128);                 // same shape: lowest attaining row
-  unsigned* sBal = sRow + 2 * 4 * 128;                                              // [16 warps][2 slabs][32 columns] ballots
+  unsigned long long* sCol = reinterpret_cast<unsigned long long*>(base + 8 * TC_BOX_BYTES + 256);   // [tile parity 2][128 columns]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int T = (n_cols + TC_BN - 1) / TC_BN;
 
-  if (warp == 0 && lane == 0) {
+  for (int i = threadIdx.x; i < 256; i += MT_THREADS) sCol[i] = 0ull;
+  if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(&maps.m1);
     tc::tma_prefetch_desc(&maps.m2);
     tc::mbar_init(a_full, 1);
     for (int i = 0; i < 2; ++i) {
       tc::mbar_init(&b_full[i], 1);
-      tc::mbar_init(&b_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], TC1_EPI_WARPS);
+      tc::mbar_init(&b_empty[i], 8);
     }
     tc::fence_barrier_init();
   }
-  if (warp == 1) {
-    tc::tmem_alloc(tmem_slot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    if (T > 0 && tc::elect_one()) {   // no column tiles: nothing may be left in flight when the CTA exits
-      // ---------------- TMA producer ----------------
+  if (warp == 8) {
+    if (T > 0 && tc::elect_one()) {
       const int arow = pair * n_pad + row0;
       tc::mbar_expect_tx(a_full, 4 * TC_BOX_BYTES);
       for (int slab = 0; slab < 2; ++slab)
@@ -604,397 +414,72 @@ __global__ void __launch_bounds__(TC1_THREADS, 1) mnn_tc_once_kernel(const __gri
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (tc::elect_one()) {
-      // ---------------- MMA issuer ----------------
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 128, TC_BN);
-      // K-blocks of x.y = hi.hi + hi.lo + lo.hi, taken from the [hi | lo] boxes of the two operands
-      constexpr int a_sel[3] = {0, 0, 1};
-      constexpr int b_sel[3] = {0, 1, 0};
-      if (T > 0) tc::mbar_wait(a_full, 0);   // (nothing was loaded when there are no column tiles)
-      for (int t = 0; t < T; ++t) {
-        const int s = t & 1, ph = (t >> 1) & 1;
-        tc::mbar_wait(&b_full[s], ph);
-        tc::mbar_wait(&acc_empty[s], ph ^ 1);
-        tc::tc_fence_after();
-#pragma unroll
-        for (int slab = 0; slab < 2; ++slab) {
-          const uint32_t d = tmem + s * 256 + slab * 128;
-#pragma unroll
-          for (int kb = 0; kb < 3; ++kb) {
-            const uint64_t da = tc::make_desc_sw128(tc::smem_u32(sA + (slab * 2 + a_sel[kb]) * TC_BOX_BYTES), 1024);
-            const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + (s * 2 + b_sel[kb]) * TC_BOX_BYTES), 1024);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              tc::umma_f16(d, da + 2 * k, db + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-        }
-        tc::umma_commit(&b_empty[s]);
-        tc::umma_commit(&acc_full[s]);
-      }
-    }
-    __syncwarp();
   } else {
-    // ---------------- epilogue: running row arg-max + column arg-max ----------------
-    // 16 warps: TMEM lane quarter q = warp & 3 (hardware rule), column quarter cq = (warp - 2) >> 2 of each 128-column slab.
-    // Four warps per scheduler: the shuffle / ballot chains of one warp are latency-bound (ncu on the 8-warp version: 42 %
-    // issue-active with 1.7 "wait" stalls per issue), so thread-level parallelism is what fills the issue slots.  To fit 576
-    // threads in the register file the chunk is re-read from TMEM for the ballots instead of being kept live.
-    const int q = warp & 3, cq = (warp - 2) >> 2, et = threadIdx.x - 64;
-    float best[2] = {-INFINITY, -INFINITY};
-    uint32_t bidx[2] = {0xffffffffu, 0xffffffffu};
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-    const bool tail = row0 + TC_ROWS > n_rows;                 // CTA-uniform: some rows are padding
-    const bool valid0 = row0 + q * 32 + lane < n_rows, valid1 = row0 + 128 + q * 32 + lane < n_rows;
-    const uint32_t gbase = (uint32_t)(row0 + q * 32);
-    const uint32_t sbal = tc::smem_u32(sBal + (warp - 2) * 64);   // this warp's ballot scratch [2 slabs][32 columns]
-    auto reduce_chunk = [&](const uint32_t (&r)[32], int col0, int slab) {
-      if (col0 + 32 <= n_cols) {
-        float m = __uint_as_float(r[0]);
+    const int slab = warp >> 2, wt = threadIdx.x & 127, et = threadIdx.x;
+    const int cq = 2 * (lane & 3);
+    float acc0[64], acc1[64];
+    unsigned long long best[4] = {0ull, 0ull, 0ull, 0ull};
+    bool rvalid[4];
 #pragma unroll
-        for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(r[j]));
-        if (m > best[slab]) {            // strict: earlier columns win ties (torch.max / argmax rule)
-          int j0 = 31;
-#pragma unroll
-          for (int j = 30; j >= 0; --j)
-            if (__uint_as_float(r[j]) == m) j0 = j;
-          best[slab] = m;
-          bidx[slab] = (uint32_t)(col0 + j0);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float v = __uint_as_float(r[j]);
-          if (col0 + j < n_cols && v > best[slab]) { best[slab] = v; bidx[slab] = (uint32_t)(col0 + j); }
-        }
-      }
-    };
-    // ballots "row attains the column maximum" for one slab of the chunk; lane `owner` parks them in shared memory
-    auto ballots = [&](const uint32_t (&r)[32], const float (&mm)[32], bool valid, uint32_t dst, int owner) {
-#pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        unsigned b[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) b[k] = __ballot_sync(0xffffffffu, valid && __uint_as_float(r[4 * j4 + k]) == mm[4 * j4 + k]);
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, %0, %1;\n\t@p st.shared.v4.u32 [%2], {%3, %4, %5, %6};\n\t}"
-                     ::"r"(lane), "r"(owner), "r"(dst + 16 * j4), "r"(b[0]), "r"(b[1]), "r"(b[2]), "r"(b[3]) : "memory");
-      }
-    };
+    for (int h = 0; h < 4; ++h) rvalid[h] = row0 + slab * 128 + tc::frag_row(wt, h) < n_rows;
+    if (T > 0) tc::mbar_wait(a_full, 0);
+    const uint32_t a_slab = tc::smem_u32(sA + slab * 2 * TC_BOX_BYTES);
     for (int t = 0; t < T; ++t) {
-      const int s = t & 1, ph = (t >> 1) & 1;
-      tc::mbar_wait(&acc_full[s], ph);
-      tc::tc_fence_after();
-      uint32_t x[32], y[32];
-      const uint32_t tb = lane_addr + s * 256 + cq * 32;
-      const int cb = t * TC_BN + cq * 32;
-      const uint32_t sval = tc::smem_u32(sVal + (s * 4 + q) * 128 + cq * 32);
-      const uint32_t srow = tc::smem_u32(sRow + (s * 4 + q) * 128 + cq * 32);
+      const int s = t & 1;
+      tc::mbar_wait(&b_full[s], (t >> 1) & 1);
+      mnn_tile_mma(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), 0);
       __syncwarp();
-      tc::tmem_ld_32x32(tb, x);            // slab 0, columns cb .. cb+31
-      tc::tmem_ld_32x32(tb + 128, y);      // slab 1, same columns
-      tc::tmem_ld_wait();
-      reduce_chunk(x, cb, 0);
-      reduce_chunk(y, cb, 1);
-      // column maxima over the warp's 64 rows: merge the slabs in-thread, transpose-reduce across the lanes
-      float a[32];
-      if (!tail) {
+      if (lane == 0) tc::mbar_arrive(&b_empty[s]);
+      mnn_row_argmax(acc0, acc1, t * TC_BN, n_cols - t * TC_BN, lane, best);
+      // column arg-max of the tile
+      unsigned long long* sc = sCol + s * 128;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) a[j] = fmaxf(__uint_as_float(x[j]), __uint_as_float(y[j]));
-      } else {                             // padding rows must not win a column
+      for (int j = 0; j < 16; ++j)
 #pragma unroll
-        for (int j = 0; j < 32; ++j)
-          a[j] = fmaxf(valid0 ? __uint_as_float(x[j]) : -INFINITY, valid1 ? __uint_as_float(y[j]) : -INFINITY);
-      }
-      col_butterfly(a, lane);              // lane l now holds the maximum of column cb + l
-      __syncwarp();
-      tc::tmem_ld_32x32(tb, x);            // re-read slab 0 for the ballots (cheaper than keeping 64 registers live)
-      asm volatile("st.shared.f32 [%0], %1;" ::"r"(sval + 4 * lane), "f"(a[0]) : "memory");
-      __syncwarp();
-      float mm[32];
+        for (int e = 0; e < 2; ++e) {
+          float m = -INFINITY;
+          int hb = -1;
 #pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4)
-        asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                     : "=f"(mm[4 * j4]), "=f"(mm[4 * j4 + 1]), "=f"(mm[4 * j4 + 2]), "=f"(mm[4 * j4 + 3])
-                     : "r"(sval + 16 * j4));   // broadcast read
-      tc::tmem_ld_wait();
-      __syncwarp();
-      tc::tmem_ld_32x32(tb + 128, y);      // slab 1 again, in flight during the slab-0 ballots
-      ballots(x, mm, valid0, sbal, 0);
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_empty[s]);   // all TMEM reads of this buffer are done
-      ballots(y, mm, valid1, sbal + 128, 1);
-      __syncwarp();
-      unsigned c0, c1;
-      asm volatile("ld.shared.u32 %0, [%1];" : "=r"(c0) : "r"(sbal + 4 * lane));
-      asm volatile("ld.shared.u32 %0, [%1];" : "=r"(c1) : "r"(sbal + 128 + 4 * lane));
-      // lowest attaining row of column `lane`: slab 0 rows precede slab 1 rows; lanes are rows in order
-      const uint32_t rfirst = c0 ? gbase + (uint32_t)(__ffs((int)c0) - 1) : (c1 ? gbase + 128u + (uint32_t)(__ffs((int)c1) - 1) : 0xffffffffu);
-      asm volatile("st.shared.u32 [%0], %1;" ::"r"(srow + 4 * lane), "r"(rfirst) : "memory");
-      asm volatile("bar.sync 1, 512;" ::: "memory");   // the tile's per-group column results are complete in parity s
-      if (et < 128 && t * TC_BN + et < n_cols) {
-        unsigned long long p = 0ull;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const unsigned r = sRow[(s * 4 + g) * 128 + et];
-          if (r != 0xffffffffu) {
-            const unsigned long long c = pack_vi(sVal[(s * 4 + g) * 128 + et], r);
-            p = c > p ? c : p;
+          for (int h = 0; h < 4; ++h) {
+            const float v = tc::frag_val(acc0, acc1, h, j, e);
+            if (rvalid[h] && v > m) { m = v; hb = h; }   // rows ascending in h: first index wins ties
           }
+          unsigned long long p = (hb >= 0) ? pack_vi(m, (uint32_t)(row0 + slab * 128 + tc::frag_row(wt, hb))) : 0ull;
+#pragma unroll
+          for (int o = 4; o <= 16; o <<= 1) {
+            const unsigned long long q = __shfl_xor_sync(0xffffffffu, p, o);
+            p = q > p ? q : p;
+          }
+          if (lane < 4 && p) atomicMax(sc + 8 * j + cq + e, p);
         }
-        if (p) atomicMax(best21 + (int64_t)pair * n2_max + t * TC_BN + et, p);
-      }
-      // parity s is written again for tile t+2, i.e. after the barrier of tile t+1, which these readers join afterwards
-    }
-    // merge the four column quarters of every row (lower column index wins ties through the packed compare)
-    unsigned long long pk[2];
-#pragma unroll
-    for (int slab = 0; slab < 2; ++slab) pk[slab] = (bidx[slab] == 0xffffffffu) ? 0ull : pack_vi(best[slab], bidx[slab]);
-    if (cq > 0) {
-      sMerge[(cq - 1) * 256 + 0 * 128 + q * 32 + lane] = pk[0];
-      sMerge[(cq - 1) * 256 + 1 * 128 + q * 32 + lane] = pk[1];
-    }
-    asm volatile("bar.sync 1, 512;" ::: "memory");     // epilogue warps only
-    if (cq == 0) {
-#pragma unroll
-      for (int slab = 0; slab < 2; ++slab) {
-        unsigned long long m = pk[slab];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const unsigned long long o = sMerge[c * 256 + slab * 128 + q * 32 + lane];
-          m = o > m ? o : m;
-        }
-        const int row = row0 + slab * 128 + q * 32 + lane;
-        if (row < n_rows) best12[(int64_t)pair * n1_max + row] = m;
+      asm volatile("bar.sync 2, 256;" ::: "memory");   // the tile's column maxima of all eight warps are in sCol[s]
+      if (et < 128) {
+        const unsigned long long p = sc[et];
+        if (p && t * TC_BN + et < n_cols) atomicMax(best21 + (int64_t)pair * n2_max + t * TC_BN + et, p);
+        sc[et] = 0ull;   // parity s is written again for tile t+2, after the barrier of tile t+1, which this thread joins later
       }
     }
-  }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc(tmem, 512);
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {
+        const int row = row0 + slab * 128 + tc::frag_row(wt, h);
+        if (row < n_rows) best12[(int64_t)pair * n1_max + row] = best[h];
+      }
+    }
   }
 }
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA-pair variant of mnn_tc_kernel (tcgen05 cta_group::2): a cluster of two CTAs = 512 rows.  The leader CTA issues UMMAs
-// with M = 256 (its 128-row slab + the peer's) and N = 256; each CTA stages HALF of every 256-column B tile (128 rows), so
-// the shared-memory operand traffic per SM is A + B/2 = 8 KB per 128-cycle MMA = 64 B/clk, half of the single-CTA kernel's
-// (A + B = 8 KB per 64-cycle MMA at N = 128, i.e. the full 128 B/clk of shared memory).  (With N = 128 per pair-MMA the
-// variant measured slower than the single-CTA kernel, 0.77 vs 0.68 ms per call.)
-// TMEM: 2 slabs x 256 columns = all 512 columns, single-buffered per slab: the epilogue of slab 0 runs under the MMAs of
-// slab 1 and vice versa, so the accumulators are still double-buffered in time.
-// Barrier topology: operand-full barriers live in the leader and collect the TMA bytes of both CTAs; stage-empty and
-// accumulator-full barriers are per CTA and are signalled by multicast tcgen05.commit; accumulator-empty lives in the leader
-// and counts the epilogue warps of both CTAs (remote mbarrier.arrive through mapa).
-constexpr int TC2_BN = 256;
-constexpr size_t TC2_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256 + 2 * 128 * 8;
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-    mnn_tc2_kernel(const __grid_constant__ TcMaps maps, const int* __restrict__ n1p, int n1_max, const int* __restrict__ n2p,
-                   int n2_max, int n_pad, unsigned long long* __restrict__ best12, unsigned long long* __restrict__ best21) {
-  const int pair = blockIdx.y, dir = blockIdx.z;
-  const int n1 = n1p ? min(n1p[pair], n1_max) : n1_max;
-  const int n2 = n2p ? min(n2p[pair], n2_max) : n2_max;
-  const int n_rows = dir ? n2 : n1, n_cols = dir ? n1 : n2;
-  const int out_stride = dir ? n2_max : n1_max;
-  unsigned long long* out = dir ? best21 : best12;
-  const CUtensorMap* mapA = dir ? &maps.m2 : &maps.m1;
-  const CUtensorMap* mapB = dir ? &maps.m1 : &maps.m2;
-  const int row0 = blockIdx.x * TC_ROWS;
-  if ((int)(blockIdx.x & ~1u) * TC_ROWS >= n_rows) return;   // cluster-uniform: both CTAs of the pair leave together
-  const uint32_t rank = tc::cluster_ctarank();
-  const bool leader = rank == 0;
-
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* sA = base;                       // [slab 2][hi, lo] 128-row boxes
-  unsigned char* sB = base + 4 * TC_BOX_BYTES;    // [stage 2][hi, lo] 128-row boxes = this CTA's half of a 256-column tile
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + 8 * TC_BOX_BYTES);
-  uint64_t* a_full = bars;         // leader: A slabs of both CTAs landed
-  uint64_t* b_full = bars + 1;     // [2 stages] leader: both halves of the B stage landed
-  uint64_t* b_empty = bars + 3;    // [2 stages] per CTA (multicast commit)
-  uint64_t* acc_full = bars + 5;   // [2 slabs] per CTA (multicast commit)
-  uint64_t* acc_empty = bars + 7;  // [2 slabs] leader: 8 epilogue warps x 2 CTAs
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  unsigned long long* sMerge = reinterpret_cast<unsigned long long*>(bars + 12);   // [2 slabs][128 rows]
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = (n_cols + TC2_BN - 1) / TC2_BN;
-
-  if (warp == 0 && lane == 0) {
-    tc::tma_prefetch_desc(mapA);
-    tc::tma_prefetch_desc(mapB);
-    tc::mbar_init(a_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&b_full[i], 1);
-      tc::mbar_init(&b_empty[i], 1);
-      tc::mbar_init(&acc_full[i], 1);
-      tc::mbar_init(&acc_empty[i], 16);
-    }
-    tc::fence_barrier_init();
-  }
-  if (warp == 1) {
-    tc::tmem_alloc_2sm(tmem_slot, 512);
-    tc::tmem_relinquish_2sm();
-  }
-  tc::tc_fence_before();
-  __syncthreads();                 // (the cluster barrier below already orders this)
-  tc::cluster_sync();              // barrier inits + TMEM allocation of both CTAs visible before any remote signal
-  tc::tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-
-  if (warp == 0) {
-    if (T > 0 && tc::elect_one()) {   // no column tiles: nothing may be left in flight when the CTA exits
-      // ---------------- TMA producer (both CTAs; bytes are reported to the leader's barriers) ----------------
-      const uint32_t a_full_l = tc::mapa_rank(tc::smem_u32(a_full), 0);
-      const int arow = pair * n_pad + row0;
-      if (leader) tc::mbar_expect_tx(a_full, 2 * 4 * TC_BOX_BYTES);
-      for (int slab = 0; slab < 2; ++slab)
-        for (int kb = 0; kb < 2; ++kb)
-          tc::tma_load_2d_2sm(sA + (slab * 2 + kb) * TC_BOX_BYTES, mapA, a_full_l, kb * 64, arow + slab * 128);
-      const int brow = pair * n_pad + (int)rank * 128;   // this CTA's half of every 256-row B tile
-      for (int t = 0; t < T; ++t) {
-        const int s = t & 1;
-        tc::mbar_wait(&b_empty[s], ((t >> 1) & 1) ^ 1);
-        if (leader) tc::mbar_expect_tx(&b_full[s], 2 * 2 * TC_BOX_BYTES);
-        const uint32_t b_full_l = tc::mapa_rank(tc::smem_u32(&b_full[s]), 0);
-        for (int kb = 0; kb < 2; ++kb)
-          tc::tma_load_2d_2sm(sB + (s * 2 + kb) * TC_BOX_BYTES, mapB, b_full_l, kb * 64, brow + t * TC2_BN);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (leader && tc::elect_one()) {
-      // ---------------- MMA issuer (leader only): M = 256 across the pair, N = 256 ----------------
-      constexpr uint32_t idesc = tc::make_idesc(/*F16*/ 0, 256, TC2_BN);
-      // K-blocks of x.y = hi.hi + hi.lo + lo.hi, taken from the [hi | lo] boxes of the two operands.  Direction 1 (A = F2,
-      // B = F1) swaps the roles of the last two blocks so both directions add the same three products in the same order and
-      // S12[i][j] == S21[j][i] bit for bit.
-      const int a_sel[3] = {0, dir ? 1 : 0, dir ? 0 : 1};
-      const int b_sel[3] = {0, dir ? 0 : 1, dir ? 1 : 0};
-      if (T > 0) tc::mbar_wait_cluster(a_full, 0);   // (nothing was loaded when there are no column tiles)
-      for (int t = 0; t < T; ++t) {
-        const int s = t & 1;
-        tc::mbar_wait_cluster(&b_full[s], (t >> 1) & 1);
-#pragma unroll
-        for (int slab = 0; slab < 2; ++slab) {
-          tc::mbar_wait_cluster(&acc_empty[slab], (t & 1) ^ 1);   // both CTAs drained this slab's accumulator (tile t-1)
-          tc::tc_fence_after();
-          const uint32_t d = tmem + slab * TC2_BN;
-#pragma unroll
-          for (int kb = 0; kb < 3; ++kb) {
-            const uint64_t da = tc::make_desc_sw128(tc::smem_u32(sA + (slab * 2 + a_sel[kb]) * TC_BOX_BYTES), 1024);
-            const uint64_t db = tc::make_desc_sw128(tc::smem_u32(sB + (s * 2 + b_sel[kb]) * TC_BOX_BYTES), 1024);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc::umma_f16_2sm(d, da + 2 * k, db + 2 * k, idesc, (kb | k) ? 1u : 0u);
-          }
-          tc::umma_commit_2sm(&acc_full[slab], 3);   // both CTAs' accumulators of (tile t, slab) are complete
-        }
-        tc::umma_commit_2sm(&b_empty[s], 3);         // both CTAs may refill their half of the stage
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue (both CTAs, own TMEM rows): running row arg-max ----------------
-    // warps 2-9: TMEM lane quarter q = warp & 3, column half hc = (warp - 2) >> 2 (128 of the slab's 256 columns)
-    const int q = warp & 3, hc = (warp - 2) >> 2;
-    float best[2] = {-INFINITY, -INFINITY};
-    uint32_t bidx[2] = {0xffffffffu, 0xffffffffu};
-    const uint32_t lane_addr = tmem + ((uint32_t)(q * 32) << 16);
-    auto reduce_chunk = [&](const uint32_t (&r)[32], int col0, int slab) {
-      if (col0 + 32 <= n_cols) {
-        float m = __uint_as_float(r[0]);
-#pragma unroll
-        for (int j = 1; j < 32; ++j) m = fmaxf(m, __uint_as_float(r[j]));
-        if (m > best[slab]) {            // strict: earlier columns win ties (torch.max / argmax rule)
-          int j0 = 31;
-#pragma unroll
-          for (int j = 30; j >= 0; --j)
-            if (__uint_as_float(r[j]) == m) j0 = j;
-          best[slab] = m;
-          bidx[slab] = (uint32_t)(col0 + j0);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float v = __uint_as_float(r[j]);
-          if (col0 + j < n_cols && v > best[slab]) { best[slab] = v; bidx[slab] = (uint32_t)(col0 + j); }
-        }
-      }
-    };
-    uint32_t acc_empty_l[2];
-    acc_empty_l[0] = tc::mapa_rank(tc::smem_u32(&acc_empty[0]), 0);
-    acc_empty_l[1] = tc::mapa_rank(tc::smem_u32(&acc_empty[1]), 0);
-    for (int t = 0; t < T; ++t) {
-#pragma unroll
-      for (int slab = 0; slab < 2; ++slab) {
-        tc::mbar_wait(&acc_full[slab], t & 1);
-        tc::tc_fence_after();
-        uint32_t ra[32], rb[32];
-        const uint32_t tb = lane_addr + slab * TC2_BN + hc * 128;
-        const int cb = t * TC2_BN + hc * 128;
-        __syncwarp();
-        tc::tmem_ld_32x32(tb, ra);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 32, rb);
-        reduce_chunk(ra, cb, slab);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 64, ra);
-        reduce_chunk(rb, cb + 32, slab);
-        tc::tmem_ld_wait();
-        __syncwarp();
-        tc::tmem_ld_32x32(tb + 96, rb);
-        reduce_chunk(ra, cb + 64, slab);
-        tc::tmem_ld_wait();
-        tc::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive_cluster(acc_empty_l[slab]);   // leader's barrier: this slab may be overwritten
-        reduce_chunk(rb, cb + 96, slab);
-      }
-    }
-    unsigned long long pk[2];
-#pragma unroll
-    for (int slab = 0; slab < 2; ++slab) pk[slab] = (bidx[slab] == 0xffffffffu) ? 0ull : pack_vi(best[slab], bidx[slab]);
-    if (hc == 1) {
-      sMerge[0 * 128 + q * 32 + lane] = pk[0];
-      sMerge[1 * 128 + q * 32 + lane] = pk[1];
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");     // epilogue warps only
-    if (hc == 0) {
-#pragma unroll
-      for (int slab = 0; slab < 2; ++slab) {
-        const unsigned long long o = sMerge[slab * 128 + q * 32 + lane];
-        const unsigned long long m = o > pk[slab] ? o : pk[slab];
-        const int row = row0 + slab * 128 + q * 32 + lane;
-        if (row < n_rows) out[(int64_t)pair * out_stride + row] = m;
-      }
-    }
-  }
-  tc::tc_fence_before();
-  tc::cluster_sync();              // the peer's shared memory / TMEM must outlive the leader's last MMA
-  if (warp == 1) {
-    tc::tc_fence_after();
-    tc::tmem_dealloc_2sm(tmem, 512);
-  }
-}
-
 
 // Both directions of the three-term scan over the full sets: the persistent kernel (default), or one CTA per (row block, pair,
-// direction) with XFEAT_MNN_ONESHOT=1 (A/B measurements).
+// direction) with `oneshot` (implementation 3) or XFEAT_MNN_ONESHOT=1.
 static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, const int* n2, int n2_max, int n_pad, int batch,
-                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st) {
-  static const bool oneshot = getenv("XFEAT_MNN_ONESHOT") != nullptr;
-  if (oneshot) {
+                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st, bool oneshot = false) {
+  static const bool oneshot_env = getenv("XFEAT_MNN_ONESHOT") != nullptr;
+  if (oneshot || oneshot_env) {
     XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
     dim3 grid(n_pad / TC_ROWS, batch, 2);
     TcMaps4 m4;
     m4.a0 = maps.m1; m4.b0 = maps.m2; m4.a1 = maps.m2; m4.b1 = maps.m1;
-    mnn_tc_kernel<<<grid, TC_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, nullptr, nullptr);
+    mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, nullptr, nullptr);
     XF_LAUNCH_CHECK();
     return XF_OK;
   }
@@ -1003,7 +488,7 @@ static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, con
   XF_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   XF_DYN_SMEM(mnn_tc_persist_kernel, TCP_SMEM);
   const int n_items = batch * 2 * (n_pad / TC_ROWS);
-  mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, TC_THREADS, TCP_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch, best12,
+  mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCP_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch, best12,
                                                                                     best21);
   XF_LAUNCH_CHECK();
   return XF_OK;
@@ -1015,7 +500,7 @@ struct MnnTcWs {
   unsigned* absmax;
   float* inv_s2;
 };
-static inline int tc_pad(int n) { return (n + 2 * TC_ROWS - 1) / (2 * TC_ROWS) * (2 * TC_ROWS); }   // a CTA pair = 512 rows
+static inline int tc_pad(int n) { return (n + 2 * TC_ROWS - 1) / (2 * TC_ROWS) * (2 * TC_ROWS); }   // 512 rows (operand layout of the API)
 
 void carve_mnn_tc(Bump& bump, int batch, int n1_max, int n2_max, MnnTcWs& ws) {
   const int n_pad = tc_pad(n1_max > n2_max ? n1_max : n2_max);
@@ -1061,11 +546,11 @@ int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, c
   MnnTcWs ws;
   carve_mnn_tc(bump, batch, n1_max, n2_max, ws);
   if (!bump.ok) {
-    set_error("mnn_match(tcgen05): workspace too small (%zu < %zu)", ws_bytes, bump.used());
+    set_error("mnn_match(tensor cores): workspace too small (%zu < %zu)", ws_bytes, bump.used());
     return XF_E_WORKSPACE;
   }
   const int n_pad = tc_pad(n1_max > n2_max ? n1_max : n2_max);
-  XF_REQUIRE((int64_t)batch * n_pad < (1ll << 31), "mnn_match(tcgen05): batch * n too large");
+  XF_REQUIRE((int64_t)batch * n_pad < (1ll << 31), "mnn_match(tensor cores): batch * n too large");
   if (!(abs_bound > 0.f)) {   // no bound from the caller: max |x| over both sets fixes the power-of-two operand scale
     XF_CUDA(cudaMemsetAsync(ws.absmax, 0, sizeof(unsigned), st));
     absmax_kernel<<<dim3(8, batch), 256, 0, st>>>(f1, n1, n1_max, stride1, ws.absmax);
@@ -1089,16 +574,10 @@ int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, c
   *best12 = ws.best12;
   *best21 = ws.best21;
   XF_CUDA(cudaMemsetAsync(ws.best21, 0, sizeof(unsigned long long) * (size_t)batch * n2_max, st));
-  if (once == 2) {   // CTA-pair kernel (cta_group::2)
-    XF_DYN_SMEM(mnn_tc2_kernel, TC2_SMEM);
-    dim3 grid2(n_pad / TC_ROWS, batch, 2);   // even by construction (n_pad is a multiple of 512): clusters of 2 along x
-    mnn_tc2_kernel<<<grid2, TC_THREADS, TC2_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, ws.best12, ws.best21);
-    XF_LAUNCH_CHECK();
-    return XF_OK;
-  }
+  if (once == 2) return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, ws.best12, ws.best21, st, true);
   if (once) {
     dim3 grid1(n_pad / TC_ROWS, batch);
-    mnn_tc_once_kernel<<<grid1, TC1_THREADS, TC1_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, ws.best12, ws.best21);
+    mnn_tc_once_kernel<<<grid1, MT_THREADS, TC1_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, ws.best12, ws.best21);
     XF_LAUNCH_CHECK();
     return XF_OK;
   }
@@ -1129,22 +608,11 @@ int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const _
   set_scalar_kernel<<<1, 1, 0, st>>>(scale, ldexpf(1.f, -2 * scale_log2));
   XF_LAUNCH_CHECK();
   *best12 = b12; *best21 = b21; *inv_s2 = scale;
-  if (pairs_kernel) {
-    TcMaps maps;
-    int rc;
-    if ((rc = make_map(&maps.m1, f1s, (uint64_t)batch * n_pad))) return rc;
-    if ((rc = make_map(&maps.m2, f2s, (uint64_t)batch * n_pad))) return rc;
-    XF_DYN_SMEM(mnn_tc2_kernel, TC2_SMEM);
-    dim3 grid2(n_pad / TC_ROWS, batch, 2);
-    mnn_tc2_kernel<<<grid2, TC_THREADS, TC2_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, b12, b21);
-    XF_LAUNCH_CHECK();
-    return XF_OK;
-  }
   TcMaps maps;
   int rc;
   if ((rc = make_map(&maps.m1, f1s, (uint64_t)batch * n_pad))) return rc;
   if ((rc = make_map(&maps.m2, f2s, (uint64_t)batch * n_pad))) return rc;
-  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st);
+  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, pairs_kernel != 0);
 }
 
 int launch_absmax(const float* f, const int* np, int n_max, int64_t stride, int batch, unsigned* out, cudaStream_t st) {
@@ -1167,7 +635,7 @@ int launch_mnn_tc_rows(const __half* a0, const __half* b0, const __half* a1, con
   if ((rc = make_map(&m4.b1, b1, (uint64_t)batch * n_pad))) return rc;
   XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
   dim3 grid(n_pad / TC_ROWS, batch, 2);
-  mnn_tc_kernel<<<grid, TC_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, rows_cnt, row_map);
+  mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, rows_cnt, row_map);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

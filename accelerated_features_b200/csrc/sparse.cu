@@ -455,7 +455,7 @@ __device__ __forceinline__ float4 bicubic4(const float* __restrict__ fb, const f
   bool interior = x0 >= 0 && x0 + 3 < Wm && y0 >= 0 && y0 + 3 < Hm;
   if (UNIFORM) interior = __all_sync(0xffffffffu, interior);
   const float4* f4 = reinterpret_cast<const float4*>(fb) + (uint32_t)l16;
-  // packed fp32 pairs (FMUL2 / FFMA2): per component  v*d, then fma(v*d, cx[j], row), then fma(row, cy[i], out)
+  // per component: v*d, then fma(v*d, cx[j], row), then fma(row, cy[i], out)
   float2 oa = make_float2(0.f, 0.f), ob = make_float2(0.f, 0.f);
   if (interior) {
     // interior keypoint (almost all): no per-tap tests, 32-bit offsets from one base pointer
@@ -511,6 +511,12 @@ __device__ __forceinline__ float4 bicubic4(const float* __restrict__ fb, const f
   return make_float4(oa.x, oa.y, ob.x, ob.y);
 }
 
+// Sum of squares of the lane's 4 channels with explicit rounding: both samplers must produce the same bits, which a
+// compiler-chosen FMA contraction does not guarantee across kernels.
+__device__ __forceinline__ float sumsq4(const float4& o) {
+  return __fmaf_rn(o.w, o.w, __fmaf_rn(o.z, o.z, __fmaf_rn(o.y, o.y, __fmul_rn(o.x, o.x))));
+}
+
 // Half a warp per output slot (b, r): lane owns 4 channels. feats: (B,Hm,Wm,64) NHWC un-normalised, den: (B,Hm,Wm).
 // The matcher's operand row of a unit-norm descriptor: x * 2^13 = hi + lo in fp16, [hi(64) | lo(64)] (mnn_tc.cu, abs_bound = 1).
 // Written next to the fp32 descriptor so xfeat_mnn_match_presplit needs no max-reduction / split pass over the descriptors.
@@ -551,7 +557,7 @@ __global__ void __launch_bounds__(256) sample_desc_kernel(const unsigned long lo
     x = (int)(lin % (uint32_t)W); y = (int)(lin / (uint32_t)W);
     o = bicubic4<false>(feats + (int64_t)b * Hm * Wm * 64, den + (int64_t)b * Hm * Wm, x, y, H, W, Hm, Wm, l16);
   }
-  float ss = o.x * o.x + o.y * o.y + o.z * o.z + o.w * o.w;
+  float ss = sumsq4(o);
 #pragma unroll
   for (int s = 8; s > 0; s >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, s);
   if (!live) return;
@@ -584,7 +590,7 @@ __global__ void __launch_bounds__(256) sample_desc_kernel(const unsigned long lo
 // by the score rank, exactly as in the generic kernel.
 // (Sharing an image between 4 CTAs of 512 threads, each repeating the bucketing, measured 321 us vs 268 us: not kept.)
 // 256-thread CTAs, SAMPLE_PARTS per image (each rebuilds the image's spatial order -- 4096 shared-memory atomics -- and samples its
-// share of it): 4 CTAs per SM by registers, and the 128 x 8 CTAs of the BASELINE batch spread over all 148 SMs, where one
+// share of it): 4 CTAs per SM by registers, and the 128 x 8 CTAs of the BASELINE batch spread over all SMs, where one
 // 1024-thread CTA per image left 20 SMs idle.
 constexpr int SAMPLE_MAX_K = 8192, SAMPLE_THREADS = 256, SAMPLE_MAX_ROWS = 512, SAMPLE_PARTS = 8;
 __global__ void __launch_bounds__(SAMPLE_THREADS, 4) sample_desc_sorted_kernel(
@@ -676,7 +682,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS, 4) sample_desc_sorted_kernel(
     const int y = (int)(((unsigned long long)lin * magic_w) >> 40), x = (int)lin - y * W;
     float4 o = bicubic4<true>(fb, db, x, y, H, W, Hm, Wm, l16);   // (an odd tail's idle half-warp samples slot 0 again and drops it)
     if (!valid) o = make_float4(0.f, 0.f, 0.f, 0.f);
-    float ss = o.x * o.x + o.y * o.y + o.z * o.z + o.w * o.w;
+    float ss = sumsq4(o);
 #pragma unroll
     for (int s = 8; s > 0; s >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, s);
     if (valid) {

@@ -159,17 +159,9 @@ struct Stem01W {
   float b1[8];
 };
 
-// Two fp32 FMAs per instruction (sm_100 FFMA2): d.xy = a.xy * b.xy + c.xy, each half an IEEE fma -- results are bit-identical to
-// two scalar fmaf calls.  The broadcast operand stays a scalar register and the weight pair comes from the constant bank through
-// the uniform datapath (LDCU), so the FMA-instruction count of the kernel halves.
+// d.xy = a * w.xy + c.xy, each half an IEEE fma (the weight pair comes from the constant bank)
 __device__ __forceinline__ float2 fma2(float a, float2 w, float2 c) {
-  float2 r;
-  const float2 aa = make_float2(a, a);
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(*reinterpret_cast<unsigned long long*>(&r))
-      : "l"(*reinterpret_cast<const unsigned long long*>(&aa)), "l"(*reinterpret_cast<const unsigned long long*>(&w)),
-        "l"(*reinterpret_cast<const unsigned long long*>(&c)));
-  return r;
+  return make_float2(__fmaf_rn(a, w.x, c.x), __fmaf_rn(a, w.y, c.y));
 }
 
 __global__ void __launch_bounds__(128) stem01_kernel(const __grid_constant__ Stem01W P, const float* __restrict__ xn,

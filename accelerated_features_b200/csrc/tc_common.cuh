@@ -1,6 +1,5 @@
-// Hand-written sm_100a primitives: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), UMMA
-// shared-memory and instruction descriptors.  Bit layouts follow the PTX ISA "tcgen05" chapter (matrix descriptor,
-// instruction descriptor for kind::f16 / kind::tf32).
+// Hand-written sm_90a primitives: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async with fp32 register
+// accumulators) and its shared-memory matrix descriptors.  Bit layouts follow the PTX ISA "wgmma" chapter.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -13,8 +12,7 @@ namespace tc {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // One elected lane of a converged warp.  Unlike `lane == 0`, ptxas knows the guarded region runs on a single thread, so
-// per-thread values feeding uniform-datapath instructions (UTCHMMA / UTMALDG operands) need no "waterfall" loop
-// (ELECT + R2UR.BROADCAST + BRA.U.ANY around every tcgen05.mma otherwise: ~100 cycles per MMA issue).
+// per-thread values feeding uniform-datapath instructions (UTMALDG operands) need no "waterfall" loop.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -75,145 +73,148 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
+// ---------------------------------------------------------------- wgmma (sm_90a)
+// D[registers] (+)= A[smem] * B[smem] for a 64-row slab, issued collectively by the four warps of one warpgroup.  Thread
+// (warp w of the group, lane l) holds rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + {0,1}:
+//   d[4j + 0..1] = row 16w + l/4, d[4j + 2..3] = row 16w + l/4 + 8.
+// Both operands K-major (no transpose), descriptors as make_desc_* below.  `accumulate` = 0 overwrites D.
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate);
+template <>
+__device__ __forceinline__ void wgmma_f16<8>(float (&d)[4], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 "
+      "{%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+template <>
+__device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// mbarrier arrives once every previously issued tcgen05.mma of this thread has completed (implies fence::before).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ---------------------------------------------------------------- CTA pair (cta_group::2, cluster of two CTAs on one TPC)
-// One tcgen05.mma issued by the leader CTA (cluster rank 0) computes M = 256: rows 0-127 from the leader's A tile and TMEM,
-// rows 128-255 from the peer's, each CTA holding HALF of the B tile (N/2 rows) at the same shared-memory offset.  Per SM the
-// operand traffic per MMA drops from A + B to A + B/2.
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {   // all threads of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {   // arrive on a (possibly remote) CTA's mbarrier
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {   // local barrier, remote arrivals
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-  } while (!ok);
-}
-// TMA load into this CTA's shared memory, completion bytes reported to the mbarrier at `bar_cluster_addr` (the leader's)
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint32_t bar_cluster_addr, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_result, uint32_t ncols) {  // same warp id in both CTAs
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {   // ONE thread of the leader CTA
+template <>
+__device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// arrives on the mbarrier at this shared-memory offset in every CTA of `cta_mask` once the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
+template <>
+__device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<80>(float (&d)[40], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(da), "l"(db), "r"(accumulate));
+}
+template <>
+__device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
 
-// 32 lanes x 32 consecutive 32-bit columns: thread t of the warp gets lane (base_lane + t), columns c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// The first N columns of a wider accumulator (the split-term GEMMs add lo.whi into the whi columns only).
+template <int N, int NW>
+__device__ __forceinline__ float (&acc_head(float (&d)[NW]))[N / 2] {
+  static_assert(N / 2 <= NW, "acc_head");
+  return *reinterpret_cast<float(*)[N / 2]>(&d[0]);
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// named barrier over the 128 threads of one warpgroup (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
+// Fragment of a 128 x 128 tile held as two 64-row slabs (d0: rows 0-63, d1: rows 64-127): element (h, j, e) of thread wt is
+// row frag_row(wt, h) (h = 0..3: r, r+8, r+64, r+72), column 8j + 2(lane%4) + e.
+__device__ __forceinline__ float frag_val(const float (&d0)[64], const float (&d1)[64], int h, int j, int e) {
+  return (h < 2) ? d0[4 * j + 2 * h + e] : d1[4 * j + 2 * (h - 2) + e];
+}
+__device__ __forceinline__ int frag_row(int wt, int h) { return 16 * (wt >> 5) + ((wt & 31) >> 2) + 8 * (h & 1) + 64 * (h >> 1); }
+
+// ---------------------------------------------------------------- accumulator -> one row per thread
+// The epilogues work on one output row per thread (rows of the 128-row tile = threads of the warpgroup).  An accumulator tile of
+// two 64-row slabs (d0: rows 0-63, d1: rows 64-127) is handed over CW columns at a time through a 16 KB shared-memory buffer:
+// 128 rows x 32 floats, 16-byte chunks XOR-swizzled by row so that both the fragment writes and the row reads are conflict-free.
+constexpr int STG_BYTES = 128 * 32 * 4;
+__device__ __forceinline__ int stg_off(int row, int col) { return row * 32 + ((((col >> 2) ^ row) & 7) << 2) + (col & 3); }
+template <int CW, int R>
+__device__ __forceinline__ void stage_write(float* stg, const float (&d0)[R], const float (&d1)[R], int c0, int wt) {
+  static_assert(CW == 16 || CW == 32, "stage_write: CW");
+  const int w = wt >> 5, l = wt & 31;
+  const int r = 16 * w + (l >> 2), cq = 2 * (l & 3);
+#pragma unroll
+  for (int jj = 0; jj < CW / 8; ++jj) {
+    const int j = c0 / 8 + jj;
+    if (4 * j + 3 < R) {
+      const int c = 8 * jj + cq;
+      *reinterpret_cast<float2*>(stg + stg_off(r, c)) = make_float2(d0[4 * j], d0[4 * j + 1]);
+      *reinterpret_cast<float2*>(stg + stg_off(r + 8, c)) = make_float2(d0[4 * j + 2], d0[4 * j + 3]);
+      *reinterpret_cast<float2*>(stg + stg_off(r + 64, c)) = make_float2(d1[4 * j], d1[4 * j + 1]);
+      *reinterpret_cast<float2*>(stg + stg_off(r + 72, c)) = make_float2(d1[4 * j + 2], d1[4 * j + 3]);
+    }
+  }
+}
+template <int CW>
+__device__ __forceinline__ void stage_read(const float* stg, int row, uint32_t (&v)[CW]) {
+#pragma unroll
+  for (int k = 0; k < CW / 4; ++k) {
+    const float4 t = *reinterpret_cast<const float4*>(stg + stg_off(row, 4 * k));
+    v[4 * k] = __float_as_uint(t.x); v[4 * k + 1] = __float_as_uint(t.y);
+    v[4 * k + 2] = __float_as_uint(t.z); v[4 * k + 3] = __float_as_uint(t.w);
+  }
+}
+// columns [c0, c0 + CW) of the tile into v[] of thread `wt` (= its row); `bar` = this warpgroup's named barrier
+template <int CW, int R>
+__device__ __forceinline__ void acc_rows(float* stg, const float (&d0)[R], const float (&d1)[R], int c0, int wt, int bar,
+                                         uint32_t (&v)[CW]) {
+  stage_write<CW>(stg, d0, d1, c0, wt);
+  wg_sync(bar);
+  stage_read<CW>(stg, wt, v);
+  wg_sync(bar);
+}
 
 // ---------------------------------------------------------------- epilogue stores
-// 256-bit global store (sm_100: STG.E.ENL2.256): one full 32-byte sector per thread and instruction.  The conv epilogues write
-// one pixel row per thread, so a warp-wide store touches 32 different rows; with 16-byte pieces every sector is written in two
-// halves by two instructions (LSU-bound: lg_throttle in profiles/r01/ncu_conv_tc_1x1_dual.md), with 32-byte pieces in one.
+// 32 bytes per thread and call as two 16-byte stores: the conv epilogues write one pixel row per thread, so a warp-wide store
+// touches 32 different rows and every 32-byte sector is written by the same thread.
 __device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&v)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]),
-               "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(v[0], v[1], v[2], v[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(v[4], v[5], v[6], v[7]);
 }
 // N fp32 values -> split fp16 row pieces: hi block at hp, lo block at lp (N halves each), x = hi + lo.  hp / lp 32-byte aligned
 // for N >= 16; N == 8: lp == hp + 8 and the 32-byte row [hi(8) | lo(8)] goes out as one store.
@@ -267,37 +268,29 @@ __device__ __forceinline__ void store_f32_row(float* op, const float (&o)[N], in
 
 // ---------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor, K-major operand, 128-byte swizzle: rows are 128 B apart inside an 8-row atom
-// (1024 B), atoms SBO apart.  Fields: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) |
-// base_offset [49,52) | layout_type [61,64) (2 = SWIZZLE_128B).
+// (1024 B), atoms SBO apart.  Fields (wgmma matrix descriptor): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
+// base_offset [49,52) | layout_type [62,64) (1 = SWIZZLE_128B, 3 = SWIZZLE_32B).
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
   d |= (uint64_t)1 << 16;                               // LBO (ignored for swizzled K-major; canonical value 1)
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;                               // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                               // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                               // SWIZZLE_128B
   return d;
 }
-// Same for 32-byte rows (SWIZZLE_32B, layout type 6): 8-row atoms of 256 B.
+// Same for 32-byte rows (SWIZZLE_32B): 8-row atoms of 256 B.
 __device__ __forceinline__ uint64_t make_desc_sw32(uint32_t smem_addr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)6 << 61;                               // SWIZZLE_32B
+  d |= (uint64_t)3 << 62;                               // SWIZZLE_32B
   return d;
 }
 template <int ROWB>
 __device__ __forceinline__ uint64_t make_desc_rows(uint32_t smem_addr) {
   return ROWB == 128 ? make_desc_sw128(smem_addr, 1024) : make_desc_sw32(smem_addr, 256);
 }
-// Instruction descriptor (kind::f16 / kind::tf32): c_format [4,6) (1 = F32), a_format [7,10), b_format [10,13)
-// (0 = F16, 1 = BF16, 2 = TF32), a_major bit 15, b_major bit 16 (0 = K-major), N>>3 [17,23), M>>4 [24,29).
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
 }  // namespace tc
 
 // Exact n / d for n < 2^22 by multiply-shift (the persistent tile loops decode tile -> (image, row, col) once per tile in

@@ -1,4 +1,4 @@
-"""Pack an XFeat state_dict into the flat fp32 blob libxfeat_sm100.so expects (csrc/layers.h).
+"""Pack an XFeat state_dict into the flat fp32 blob libxfeat_sm90.so expects (csrc/layers.h).
 
 Every conv / linear is stored as W[tap][cin][cout] (cout fastest) followed by bias[cout], with the eval-mode
 BatchNorm(affine=False, eps=1e-5) that follows it folded in (model.py:12-25, 97-111):

@@ -1,7 +1,7 @@
-"""Drop-in replacement for `modules.xfeat.XFeat` (verlab/accelerated_features) on NVIDIA B200.
+"""Drop-in replacement for `modules.xfeat.XFeat` (verlab/accelerated_features) on NVIDIA H100.
 
 Same constructor, method names, argument meaning, return types and error behaviour as the reference class
-(modules/xfeat.py), but every operation of the hot path runs in libxfeat_sm100.so (hand-written sm_100a CUDA kernels
+(modules/xfeat.py), but every operation of the hot path runs in libxfeat_sm90.so (hand-written sm_90a CUDA kernels
 behind the C-ABI of include/xfeat_b200.h).  PyTorch is used for device memory, streams and the final slicing only.
 There is no CPU / eager fallback: without a CUDA device and the built library the constructor raises.
 
@@ -107,14 +107,14 @@ class _Net(torch.nn.Module):
 
 
 class XFeat(torch.nn.Module):
-    """B200-native XFeat inference (sparse `detectAndCompute` / `match_xfeat`, semi-dense `match_xfeat_star`)."""
+    """H100-native XFeat inference (sparse `detectAndCompute` / `match_xfeat`, semi-dense `match_xfeat_star`)."""
 
     def __init__(self, weights=_weights.DEFAULT_WEIGHTS, top_k: int = 4096, detection_threshold: float = 0.05,
                  device: Optional[int] = None):
         # reference: xfeat.py:23-46.  `weights`: path (.pt/.npz), state_dict mapping, or None (random init)
         super().__init__()
         if not torch.cuda.is_available():
-            raise RuntimeError("accelerated_features_b200.XFeat needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("accelerated_features_b200.XFeat needs a CUDA device (sm_90a); there is no CPU fallback")
         self._lib = _lib.load()
         dev_index = torch.cuda.current_device() if device is None else int(device)
         self.dev = torch.device("cuda", dev_index)

@@ -11,7 +11,12 @@ A "step" is one pass of the hot path over one batch of 64 synthetic image pairs 
 `value`   : pairs/s with the inputs already resident in HBM (CUDA events around K steps, max over ranks).
 `e2e`     : pairs/s through the PUBLIC API (XFeat.match_xfeat_stream / XFeat.match_xfeat_star) with HOST (pinned) inputs: H2D of
             both image sets and D2H of the results inside the timed region.
-`roofline`: the dominant kernel: algorithmic FLOPs / its CUDA-event time inside the timed steps, against MEASURED_PEAKS.json.
+`roofline`: the dominant kernel: algorithmic FLOPs / its CUDA-event time inside the timed steps, against MEASURED_PEAKS.json
+            (else the H100 SXM data-sheet figure: 989 TFLOP/s dense BF16).
+`--dump-outputs DIR`: after the timed steps, the last step's results as DIR/<name>.npy (float32 / float64): sparse -- the matched
+            keypoints of both sides (pairs x top_k x 2, rows past the pair's match count zeroed) and the per-pair match / keypoint
+            counts; star -- the refined matches (pairs x top_k x 4, rows past the pair's count zeroed) and the counts.  The inputs
+            are seeded, so two builds run with the same arguments can be compared output for output.
 `cpu_baseline` / `--impl reference`: the reference's own modules/xfeat.py (byte-compiled into oracle/_ref by
             oracle/build_ref.py), CUDA hidden, all host threads, same workload shape; falls back to the oracle PORT only if
             oracle/_ref is missing, and says so in `kind`.
@@ -45,7 +50,7 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -195,16 +200,27 @@ def run_reference(args):
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU arm
 # ---------------------------------------------------------------------------------------------------------------------
-def load_ncu(name):
-    for rnd in ("r02", "r01"):
-        try:
-            with open(os.path.join(ROOT, "profiles", rnd, name)) as f:
-                d = json.load(f)
-            d["profile"] = f"profiles/{rnd}/{name}"
-            return d
-        except Exception:
-            pass
-    return None
+def dump_outputs(path: str, out, star: bool):
+    """The results of one step of the timed path, as a caller would receive them (see the module docstring)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+
+    def rows(x, n):   # (pairs, rows, k): zero the rows past each pair's count (they are never written)
+        x = x.float().cpu()
+        keep = torch.arange(x.shape[1])[None, :] < n.cpu().long()[:, None]
+        return (x * keep[..., None]).numpy()
+
+    if star:
+        m, n_ref, cnt = out
+        arrays = {"matches": rows(m, n_ref), "n_refined": n_ref, "n_coarse": cnt}
+    else:
+        mk0, mk1, cnt, n1, n2 = out
+        arrays = {"mkpts0": rows(mk0, cnt), "mkpts1": rows(mk1, cnt), "n_matches": cnt, "n_kpts0": n1, "n_kpts1": n2}
+    for name, a in arrays.items():
+        if isinstance(a, torch.Tensor):
+            a = a.cpu().numpy().astype(np.float64)
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def run_gpu(args):
@@ -288,6 +304,8 @@ def run_gpu(args):
         out = step_resident(record=True)
     t1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, star)
     launches = lib.xfeat_launch_count() - launches0
     ms_total = t0.elapsed_time(t1)
     dom_ms = statistics.mean(a.elapsed_time(b) for a, b in dom_events)
@@ -364,24 +382,23 @@ def run_gpu(args):
         pk, pk_kind = peaks()
         pairs = BATCH * world * args.steps
         value = pairs / (ms_total / 1e3)
-        peak = pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
+        peak = pk["bf16_tflops"]
         if star:
             # dominant stage: dual-scale dense extraction = 2 x xfeat_net at 0.6x and 1.3x (SURVEY 8d: 21.5 GFLOP per 1280x960 image)
             flops = 2.0 * BATCH * 21.50e9
-            kname = ("dense extraction of both image sets (resize + xfeat_net at 768x576 and 1664x1248 + top-k/gather): tcgen05 split-fp16 "
+            kname = ("dense extraction of both image sets (resize + xfeat_net at 768x576 and 1664x1248 + top-k/gather): wgmma split-fp16 "
                      "implicit-GEMM convolutions dominate")
             cfg_extra = {"mean_coarse_matches": float(out[2].float().mean()), "mean_refined": float(out[1].float().mean())}
             d2h = int(BATCH * 4)
-            ncu, note = None, "algorithmic conv FLOPs (each MAC once) of both image sets / event time of the extraction stage"
+            note = "algorithmic conv FLOPs (each MAC once) of both image sets / event time of the extraction stage"
         else:
             flops = 2.0 * 64.0 * float((out[3].double() * out[4].double()).sum())
             impl = lib.xfeat_get_mnn_impl()
             kname = (f"xfeat_mnn_match_presplit (impl {impl}): mnn_tc_persist_kernel, fused D1.D2^T (3-term split fp16) + row arg-max, both "
-                     "directions, tcgen05; timed call also contains the finalize kernel")
+                     "directions, wgmma; timed call also contains the finalize kernel")
             cfg_extra = {"mean_keypoints": [float(out[3].float().mean()), float(out[4].float().mean())],
                          "mean_matches_per_pair": float(out[2].float().mean())}
             d2h = int(2 * BATCH * TOPK * 2 * 4 + BATCH * 4)
-            ncu = load_ncu("ncu_mnn.json")
             note = "achieved counts each MAC of ONE similarity matrix once (SURVEY 8d); both scan directions and precision passes are overhead"
         achieved = flops / (dom_ms / 1e3) / 1e12
         line = {
@@ -389,7 +406,7 @@ def run_gpu(args):
             "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic randn (reference minimal_example.py style), pretrained XFeat weights",
             "config": {"workload": cfg["workload"], "pairs_per_gpu": BATCH, "top_k": TOPK,
-                       "l2": f"inputs {2 * h1.numel() * 4 // 1000000} MB/step > 126 MB L2", "parallelism": f"pair-sharded x{world}",
+                       "l2": f"inputs {2 * h1.numel() * 4 // 1000000} MB/step > 50 MB L2", "parallelism": f"pair-sharded x{world}",
                        **cfg_extra},
             "e2e": {"value": pairs / (e2e_ms / 1e3), "unit": "pairs/s", "h2d_bytes_per_step": int(2 * h1.numel() * 4),
                     "d2h_bytes_per_step": d2h, "ms_per_step": e2e_ms / args.steps, "h2d_only_gbs": h2d_gbs,
@@ -399,9 +416,8 @@ def run_gpu(args):
             "gpu_launches": int(launches),
             "clocks": clocks,
             "roofline": {"kernel": kname, "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": achieved / peak, "peak_kind": f"{pk_kind} bf16 dense, sustained", "ms_per_launch": dom_ms,
-                         "note": note,
-                         "traffic": (ncu["dram_bytes_read"] + ncu["dram_bytes_write"]) if ncu else None, "ncu": ncu},
+                         "frac": achieved / peak, "peak_kind": f"{pk_kind}, bf16 dense", "ms_per_launch": dom_ms,
+                         "note": note},
         }
         if e2e_u8_ms:
             line["e2e_u8"] = {"value": pairs / (e2e_u8_ms / 1e3), "unit": "pairs/s", "h2d_bytes_per_step": hu_bytes,
@@ -425,12 +441,15 @@ def main():
         return
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="sparse", choices=sorted(CONFIGS))
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * xfeat_b200.h -- C-ABI of libxfeat_sm100.so: the XFeat inference hot path as sm_100a CUDA kernels.
+ * xfeat_b200.h -- C-ABI of libxfeat_sm90.so: the XFeat inference hot path as sm_90a CUDA kernels.
  *
  * The reference (verlab/accelerated_features) has no FFI / plugin interface of its own: its boundary is the
  * Python surface of modules/xfeat.py (SURVEY.md section 8b).  Each entry point below replaces the ATen call
@@ -94,7 +94,7 @@ XF_API int xfeat_preprocess_scaled(const void* d_img, int dtype, int B, int C, i
                             int H, int W, float scale_h, float scale_w, float* d_xn, double* d_stats, void* stream);
 
 /* Implementation switch of the conv layers inside xfeat_net (process-wide): 0 = fp32 CUDA-core kernels everywhere,
- * 1 = tcgen05 tensor-core kernels (split-fp16 operands, fp32 accumulation in TMEM), 2 = as 1 plus halo-patch operand
+ * 1 = wgmma tensor-core kernels (split-fp16 operands, fp32 register accumulation), 2 = as 1 plus halo-patch operand
  * reuse for the 3x3 stride-1 layers.  xfeat_set_halo_desc_mode is a bring-up knob of mode 2 (1 = PTX base_offset rule). */
 XF_API void xfeat_set_halo_desc_mode(int mode);
 XF_API void xfeat_set_conv_impl(int impl);
@@ -144,9 +144,9 @@ XF_API int xfeat_detect_dense(xfeat_ctx* ctx, const float* d_feats, const float*
                        float* d_kpts, float* d_desc, float* d_scales, int32_t* d_topk_idx, void* d_ws, size_t ws_bytes,
                        void* stream);
 
-/* Implementation switch of xfeat_mnn_match (process-wide): 0 = fp32 CUDA-core kernel; 1 = tcgen05 tensor-core kernel
- * (split-fp16 operands, fp32 accumulation in TMEM, one three-term GEMM per direction; default); 2 = tcgen05, single GEMM with the
- * column arg-max reduced in the epilogue; 3 = implementation 1 on CTA pairs (tcgen05 cta_group::2); 4 = filter +
+/* Implementation switch of xfeat_mnn_match (process-wide): 0 = fp32 CUDA-core kernel; 1 = wgmma tensor-core kernel
+ * (split-fp16 operands, fp32 register accumulation, one three-term GEMM per direction; default); 2 = wgmma, single GEMM with the
+ * column arg-max reduced in the epilogue; 3 = implementation 1, one CTA per work item; 4 = filter +
  * exact re-score: one fp16 pass per direction tracking top-1 / top-2, then implementation 1's kernel only on the rows whose
  * gap is within the rounding bound of the dropped split terms.  All honour the same tie rule; 1-4 return identical results.
  * Values outside 0..4 are clamped. */

@@ -1,4 +1,4 @@
-"""CPU-side checks of the C-ABI boundary: the library builds for sm_100a, loads, and exports exactly the symbols
+"""CPU-side checks of the C-ABI boundary: the library builds for sm_90a, loads, and exports exactly the symbols
 include/xfeat_b200.h declares (no compute calls: there is no GPU here)."""
 import ctypes
 import os
@@ -44,10 +44,10 @@ def test_library_loads_and_reports(lib_path):
     assert lib.xfeat_launch_count() == 0
 
 
-def test_sass_is_sm100a_only(lib_path):
+def test_sass_is_sm90a_only(lib_path):
     out = subprocess.run(["cuobjdump", "--list-elf", lib_path], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_product_never_imports_oracle():

@@ -1,4 +1,4 @@
-"""Halo-patch variant of the tcgen05 conv (3x3 stride 1): taps addressed by shifting the shared-memory descriptor."""
+"""Halo-patch variant of the wgmma conv (3x3 stride 1): taps addressed by shifting the shared-memory descriptor."""
 import contextlib
 
 import pytest

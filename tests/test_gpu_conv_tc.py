@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv (64->64, 3x3 / 1x1, stride 1; split-fp16 operands, fp32 accumulation) against the oracle,
+"""wgmma implicit-GEMM conv (64->64, 3x3 / 1x1, stride 1; split-fp16 operands, fp32 accumulation) against the oracle,
 layer by layer, through the whole network, and end to end."""
 import contextlib
 
@@ -97,7 +97,7 @@ def test_net_tc_vs_oracle(xf, oracle_state, golden, assets_vga, which, impl):
     e_log = (logits.permute(0, 3, 1, 2).cpu() - st["kpt_logits"]).abs().max().item()
     e_rel = (rel.cpu() - st["reliability"][:, 0]).abs().max().item()
     e_heat = (heat.cpu() - orc.kpts_heatmap(st["kpt_logits"])[:, 0]).abs().max().item()
-    print(f"[{which}] tcgen05 impl {impl}: feats rel {e_feats:.2e} logits abs {e_log:.2e} reliability abs {e_rel:.2e} heat abs {e_heat:.2e}; "
+    print(f"[{which}] tensor-core impl {impl}: feats rel {e_feats:.2e} logits abs {e_log:.2e} reliability abs {e_rel:.2e} heat abs {e_heat:.2e}; "
           f"vs simt feats rel {relerr(feats, feats0):.2e}")
     # 3-term fp16 split carries 22 mantissa bits per operand (fp32: 24): a few 1e-5 after ~20 layers, 1e-3 is the budget
     assert e_feats < 1e-4 and e_log < 5e-4 and e_rel < 5e-5 and e_heat < 5e-5
@@ -119,13 +119,13 @@ def test_e2e_tc_detect_and_match(xf, oracle_state, assets_vga, golden):
         wi = {(float(a), float(c)): i for i, (a, c) in enumerate(wk)}
         ia = np.array([gi[c] for c in common]); ib = np.array([wi[c] for c in common])
         derr = np.abs(got[b]["descriptors"].cpu().numpy()[ia] - want[b]["descriptors"].numpy()[ib]).max()
-        print(f"tcgen05 convs, image {b}: common keypoints {len(common)}/{len(wk)} ({frac:.4f}), desc max err {derr:.2e}")
+        print(f"tensor-core convs, image {b}: common keypoints {len(common)}/{len(wk)} ({frac:.4f}), desc max err {derr:.2e}")
         assert frac >= 0.995 and derr < 1e-3
     g = golden("g1_sparse_vga.npz")
     wantm = {(float(a), float(b), float(c), float(d)) for (a, b), (c, d) in zip(g["mkpts0"], g["mkpts1"])}
     gotm = {(float(a), float(b), float(c), float(d)) for (a, b), (c, d) in zip(mk0, mk1)}
     frac = len(wantm & gotm) / len(wantm)
-    print(f"tcgen05 convs: matches {len(gotm)} vs golden {len(wantm)}, common {frac:.4f}")
+    print(f"tensor-core convs: matches {len(gotm)} vs golden {len(wantm)}, common {frac:.4f}")
     assert frac >= 0.98
 
 
@@ -137,5 +137,5 @@ def test_star_tc(xf, assets_vga, golden):
     want0, want1 = g["b1_mk0"], g["b1_mk1"]
     wd = {(float(r[0]), float(r[1])): s for r, s in zip(want1, want0)}
     hit = sum(1 for s, r in zip(a0, a1) if (float(r[0]), float(r[1])) in wd and np.abs(wd[(float(r[0]), float(r[1]))] - s).max() < 0.05)
-    print(f"star (tcgen05 convs): {len(a0)} vs {len(want0)} refined matches, agreeing {hit}")
+    print(f"star (tensor-core convs): {len(a0)} vs {len(want0)} refined matches, agreeing {hit}")
     assert hit >= 0.95 * len(want0)

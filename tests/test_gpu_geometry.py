@@ -158,7 +158,7 @@ def test_batched_harness_equals_per_pair_and_reference_auc(xf, oracle_state, ass
 
     mine = run_pose_benchmark(match_pairs, samples, ransac_thr=2.5, batch_size=3, pose_fn=pose_fn)
     theirs = run_pose_benchmark(ref_matcher, samples, ransac_thr=2.5, batch_size=1, pose_fn=pose_fn)
-    print("AUC batched B200:", {k: round(v, 4) for k, v in mine.items() if k != "pairs"})
+    print("AUC batched GPU:", {k: round(v, 4) for k, v in mine.items() if k != "pairs"})
     print("AUC reference   :", {k: round(v, 4) for k, v in theirs.items() if k != "pairs"})
     from tests.parity_util import record
     record("eval_harness_auc", b200={k: v for k, v in mine.items() if k != "pairs"},

@@ -1,4 +1,4 @@
-"""tcgen05 (tensor-core, split-fp16) implementation of xfeat_mnn_match against the CPU oracle.
+"""wgmma (tensor-core, split-fp16) implementation of xfeat_mnn_match against the CPU oracle.
 
 The tensor-core scan computes S = hi.hi + hi.lo + lo.hi with fp32 accumulation: agreement with the fp32 oracle is exact
 except where the arg-max is separated from the runner-up by less than accumulation noise; any difference must be
@@ -67,7 +67,7 @@ def run(xf, f1, f2, thr):
     return i0.cpu().numpy(), i1.cpu().numpy()
 
 
-TC_IMPLS = [4, 1, 2, 3]   # 4: filter + exact re-score (default), 1: one 3-term GEMM per direction, 2: single GEMM (row + column arg-max), 3: 1 on CTA pairs
+TC_IMPLS = [4, 1, 2, 3]   # 4: filter + exact re-score (default), 1: one 3-term GEMM per direction, 2: single GEMM (row + column arg-max), 3: 1 with one CTA per work item
 
 
 @pytest.mark.parametrize("impl", TC_IMPLS)
@@ -122,7 +122,7 @@ def test_tc_equals_simt_on_real_descriptors(xf, assets_vga, impl):
         b0, b1 = xf.match(d0, d1, -1)
         c0, c1 = xf.match(d0, d1, 0.82)
     nd = check_modulo_ties(d0.cpu(), d1.cpu(), (b0.cpu().numpy(), b1.cpu().numpy()), (a0.cpu().numpy(), a1.cpu().numpy()))
-    print(f"asset pair: simt {len(a0)} matches, tcgen05 {len(b0)}, differing pairs {nd}; 0.82 -> {len(c0)}")
+    print(f"asset pair: simt {len(a0)} matches, tensor cores {len(b0)}, differing pairs {nd}; 0.82 -> {len(c0)}")
     w0, w1 = orc.mnn_match(d0.cpu(), d1.cpu(), 0.82)
     check_modulo_ties(d0.cpu(), d1.cpu(), (c0.cpu().numpy(), c1.cpu().numpy()), (w0.numpy(), w1.numpy()))
     assert nd <= 4
