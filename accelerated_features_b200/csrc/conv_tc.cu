@@ -655,11 +655,16 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
 
 }  // namespace xf
 
-// Test hook: one eligible layer through the tensor-core kernel with fp32 NHWC in/out (the split of the input runs first).
-extern "C" int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out,
-                                         void* d_scratch, size_t scratch_bytes, void* stream) {
-  XF_REQUIRE(ctx && d_in && d_out && d_scratch && layer >= 0 && layer < xf::L_COUNT, "debug_conv_layer_tc: bad arguments");
+// Test hooks: one eligible layer through the tensor-core kernel from fp32 NHWC input (the split of the input runs first); the
+// _ex form also writes the split output the next layer reads and takes block1.3's skip input.
+extern "C" int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W,
+                                            float* d_out_f32, void* d_out_split, const float* d_skip_xn, void* d_scratch,
+                                            size_t scratch_bytes, void* stream) {
+  XF_REQUIRE(ctx && d_in && (d_out_f32 || d_out_split) && d_scratch && layer >= 0 && layer < xf::L_COUNT && B > 0 && H > 0 &&
+                 W > 0,
+             "debug_conv_layer_tc: bad arguments");
   XF_REQUIRE(xf::conv_tc_eligible(layer), "debug_conv_layer_tc: layer %d has no tensor-core configuration", layer);
+  XF_REQUIRE(!d_skip_xn || layer == xf::L_B1_3, "debug_conv_layer_tc: the skip input belongs to block1.3 only");
   const int cin = xf::kLayers[layer].cin, cinp = cin <= 8 ? 8 : (cin <= 32 ? 32 : (cin <= 64 ? 64 : 128));
   const int64_t npix = (int64_t)B * H * W;
   XF_REQUIRE(scratch_bytes >= (size_t)npix * 4 * cinp, "debug_conv_layer_tc: scratch must hold B*H*W*%d bytes", 4 * cinp);
@@ -667,5 +672,11 @@ extern "C" int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float*
   cudaStream_t st = (cudaStream_t)stream;
   int rc = xf::launch_split_nhwc(d_in, (__half*)d_scratch, npix, cin, cinp, st);
   if (rc) return rc;
-  return xf::launch_conv_tc(ctx, layer, (const __half*)d_scratch, B, H, W, nullptr, d_out, st, nullptr);
+  return xf::launch_conv_tc(ctx, layer, (const __half*)d_scratch, B, H, W, (__half*)d_out_split, d_out_f32, st, d_skip_xn);
+}
+
+extern "C" int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out,
+                                         void* d_scratch, size_t scratch_bytes, void* stream) {
+  XF_REQUIRE(d_out, "debug_conv_layer_tc: bad arguments");
+  return xfeat_debug_conv_layer_tc_ex(ctx, layer, d_in, B, H, W, d_out, nullptr, nullptr, d_scratch, scratch_bytes, stream);
 }

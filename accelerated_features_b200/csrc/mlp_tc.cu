@@ -4,7 +4,8 @@
 // the batch at once (rows = sum of the per-pair match counts, read from device memory: tiles past the live rows are never
 // scheduled).  Operands are split as everywhere in this library: x = hi + lo (fp16), w * 2^k = whi + wlo,
 //      y = (hi.whi + hi.wlo + lo.whi) * 2^-k + b          (fp32 accumulation in registers)
-// so the result is fp32-equivalent (tests: 1e-3 of the logit range; refined coordinates 2e-3 px).  Activations travel between
+// so the result is fp32-equivalent (tests: 6e-4 absolute on the logits, at most 1/5 of the error with any one term dropped, and
+// 5e-4 px on the sub-pixel offsets; tests/split_ref.py).  Activations travel between
 // the layers already split, rows of [hi(K) | lo(K)] halves, written by the producing epilogue.
 //   warp 4: TMA producer, one 64-channel K block per stage {A hi, A lo, W hi, W lo};  warps 0-3: one warpgroup that issues, per
 //   K block and 64-row slab, 4 x wgmma(64 x 2NT x 16) hi.[whi ; wlo] + 4 x wgmma(64 x NT x 16) lo.whi, then runs the epilogue

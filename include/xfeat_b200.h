@@ -268,6 +268,17 @@ XF_API int xfeat_debug_conv_layer(xfeat_ctx* ctx, int layer, const float* d_in, 
 XF_API int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out,
                                      void* d_scratch, size_t scratch_bytes, void* stream);
 
+/* Test hook: xfeat_debug_conv_layer_tc for any tensor-core layer, with the outputs the network passes on.  Follows
+ * xfeat_set_conv_impl exactly as xfeat_net does.  d_in (B,H,W,Cin) fp32 NHWC is split into d_scratch (>= B*H*W*4*Cinp bytes,
+ * Cinp = Cin rounded up to 8, 32, 64 or 128) first.  Outputs, at least one of them (Ho = H/stride, Wo = W/stride):
+ *   d_out_f32 (B,Ho,Wo,Cout) fp32, or NULL;
+ *   d_out_split (B,Ho,Wo,2*Cs) fp16 [hi(Cs) | lo(Cs)], Cs = 8 for block1.2, 32 for Cout = 24, else Cout; or NULL.
+ * d_skip_xn: block1.3 only, the normalised gray image (B,4*Ho,4*Wo) fp32 whose AvgPool2d(4) . skip1 is added (model.py:140);
+ * NULL for none. */
+XF_API int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out_f32,
+                                        void* d_out_split, const float* d_skip_xn, void* d_scratch, size_t scratch_bytes,
+                                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,7 @@ import torch.nn.functional as F
 pytestmark = pytest.mark.gpu
 
 from oracle import xfeat_oracle as orc  # noqa: E402
+from tests import split_ref  # noqa: E402
 
 
 @pytest.fixture(scope="module")
@@ -76,7 +77,7 @@ def test_fine_matcher_and_subpix(xf, oracle_state):
     want = orc.fine_matcher(oracle_state, x)
     got = xf.net.fine_matcher(x.cuda())
     assert got.shape == (300, 64)
-    assert (got.cpu() - want).abs().max().item() < 1e-3 * max(1.0, float(want.abs().max()))
+    assert (got.cpu() - want).abs().max().item() < split_ref.FINE_MATCHER_TOL   # sees a dropped split term (test_split_error_model)
     want_xy = orc.subpix_softmax2d(want.view(-1, 8, 8))
     got_xy = xf.subpix_softmax2d(want.view(-1, 8, 8).cuda())
     assert (got_xy.cpu() - want_xy).abs().max().item() < 1e-5
