@@ -54,6 +54,13 @@ SIGNATURES = {
     "xfeat_ransac_workspace_bytes": (c_sz, [c_i, c_i]),
     "xfeat_ransac_homography": (c_i, [c_p, c_p, c_p, c_i, c_i, c_f, c_i, C.c_uint32, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_ransac_essential": (c_i, [c_p, c_p, c_p, c_i, c_i, c_f, c_i, C.c_uint32, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_lg_packed_weight_floats": (c_sz, []),
+    "xfeat_lg_create": (c_i, [C.POINTER(c_p), c_i, c_p, c_sz]),
+    "xfeat_lg_destroy": (None, [c_p]),
+    "xfeat_lg_workspace_bytes": (c_sz, [c_i, c_i]),
+    "xfeat_lg_match": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_f, c_i, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_lg_debug": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_lg_debug_attention": (c_i, [c_p, c_p, c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p]),
     "xfeat_debug_conv_layer": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p]),
     "xfeat_debug_conv_layer_tc": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
     "xfeat_debug_conv_layer_tc_ex": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz, c_p]),

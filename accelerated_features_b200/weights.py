@@ -92,6 +92,90 @@ def fold_layer(sd: Mapping[str, np.ndarray], conv: str, bn):
     return np.ascontiguousarray(wk, dtype=np.float32), b.astype(np.float32)
 
 
+def _pad4(chunks, arr):
+    chunks.append(np.asarray(arr, np.float32).reshape(-1))
+    if chunks[-1].size % 4:
+        chunks.append(np.zeros((-chunks[-1].size) % 4, np.float32))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# LighterGlue (modules/lighterglue.py): the `matcher.*` part of weights/xfeat-lighterglue.pt
+# ---------------------------------------------------------------------------------------------------------------------
+# The matcher's weights are not shipped with the package: they are the published weights/xfeat-lighterglue.pt of the reference
+# (the reference itself downloads them when its checkout lacks the file, lighterglue.py:35-38).  Put that file here, or pass its
+# path to XFeat(lighterglue_weights=...).
+LG_DEFAULT_WEIGHTS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "weights", "xfeat-lighterglue.pt")
+LG_LAYERS = 6
+LG_DIM = 96
+
+
+def save_lighterglue_state(pt_path: str, out_path: str) -> Dict[str, np.ndarray]:
+    """Re-save the published `matcher.*` state as .npz with lighterglue.py:40-46's renaming (`self_attn.{i}` ->
+    `transformers.{i}.self_attn`, same for cross_attn, `matcher.` prefix dropped)."""
+    sd = load_lighterglue_state(pt_path)
+    np.savez(out_path, **{k: np.ascontiguousarray(v, dtype=np.float32) for k, v in sd.items()})
+    return sd
+
+
+def load_lighterglue_state(weights=LG_DEFAULT_WEIGHTS) -> Dict[str, np.ndarray]:
+    """The matcher state from the published .pt (extractor + matcher; the `matcher.*` part is kept, renamed), a re-saved .npz,
+    or a mapping with the renamed keys."""
+    if isinstance(weights, (str, os.PathLike)) and not os.path.exists(weights):
+        raise FileNotFoundError(
+            f"LighterGlue weights not found at {os.fspath(weights)}: place the published weights/xfeat-lighterglue.pt of "
+            "verlab/accelerated_features there, or pass its path as XFeat(lighterglue_weights=...)")
+    sd = load_state_dict(weights)
+    if any(k.startswith("matcher.") for k in sd):
+        out = {}
+        for k, v in sd.items():
+            if not k.startswith("matcher."):
+                continue
+            for i in range(LG_LAYERS):
+                k = k.replace(f"self_attn.{i}", f"transformers.{i}.self_attn").replace(f"cross_attn.{i}",
+                                                                                     f"transformers.{i}.cross_attn")
+            out[k[len("matcher."):]] = v
+        sd = out
+    return sd
+
+
+def pack_lighterglue(sd: Mapping[str, np.ndarray]) -> np.ndarray:
+    """Flat fp32 blob of xfeat_lg_create (csrc/lighterglue.cu, `LgWeights`).  Every linear is stored as W[in][out] (out fastest)
+    followed by its bias, each array padded to 4 floats.  Only row permutations, no arithmetic: Wqkv is de-interleaved from
+    (q, k, v) = output rows (3i, 3i+1, 3i+2) into [q | k | v], and each cross block's to_qk and to_v are stored as one
+    96 -> 192 linear [qk | v]."""
+    g = lambda k: _np(sd[k]).astype(np.float32)  # noqa: E731
+    lin = lambda w: np.ascontiguousarray(w.T)     # noqa: E731  (out,in) -> [in][out]
+    chunks = []
+    _pad4(chunks, lin(g("input_proj.weight")))
+    _pad4(chunks, g("input_proj.bias"))
+    _pad4(chunks, lin(g("posenc.Wr.weight")))                                   # [2][48]
+    for i in range(LG_LAYERS):
+        p = f"transformers.{i}."
+        w, b = g(p + "self_attn.Wqkv.weight"), g(p + "self_attn.Wqkv.bias")
+        perm = np.concatenate([np.arange(LG_DIM) * 3 + c for c in range(3)])
+        _pad4(chunks, lin(w[perm]))
+        _pad4(chunks, b[perm])
+        _pad4(chunks, lin(g(p + "self_attn.out_proj.weight")))
+        _pad4(chunks, g(p + "self_attn.out_proj.bias"))
+        for blk in ("self_attn", "cross_attn"):
+            if blk == "cross_attn":
+                _pad4(chunks, lin(np.concatenate([g(p + "cross_attn.to_qk.weight"), g(p + "cross_attn.to_v.weight")])))
+                _pad4(chunks, np.concatenate([g(p + "cross_attn.to_qk.bias"), g(p + "cross_attn.to_v.bias")]))
+                _pad4(chunks, lin(g(p + "cross_attn.to_out.weight")))
+                _pad4(chunks, g(p + "cross_attn.to_out.bias"))
+            q = p + blk + ".ffn."
+            for name in ("0.weight", "0.bias", "1.weight", "1.bias", "3.weight", "3.bias"):
+                a = g(q + name)
+                _pad4(chunks, lin(a) if a.ndim == 2 else a)
+    for i in range(LG_LAYERS):
+        p = f"log_assignment.{i}."
+        _pad4(chunks, lin(g(p + "final_proj.weight")))
+        _pad4(chunks, g(p + "final_proj.bias"))
+        _pad4(chunks, g(p + "matchability.weight"))
+        _pad4(chunks, g(p + "matchability.bias"))
+    return np.ascontiguousarray(np.concatenate(chunks), dtype=np.float32)
+
+
 def pack_weights(sd: Mapping[str, np.ndarray]) -> np.ndarray:
     chunks = []
     pad4 = lambda n: (-n) % 4  # noqa: E731

@@ -6,7 +6,8 @@ behind the C-ABI of include/xfeat_b200.h).  PyTorch is used for device memory, s
 There is no CPU / eager fallback: without a CUDA device and the built library the constructor raises.
 
 Beyond the reference surface: `match_xfeat_batch` (batched match_xfeat) and `match_xfeat_stream` (pinned, double-buffered
-host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1).
+host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match_lighterglue_batch` and
+`match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu).
 """
 from __future__ import annotations
 
@@ -106,12 +107,38 @@ class _Net(torch.nn.Module):
         return feats.permute(0, 3, 1, 2), logits.permute(0, 3, 1, 2), rel.unsqueeze(1)
 
 
+# LightGlue prunes an image only while it has more points than this; 1536 is upstream's threshold on CUDA with
+# scaled-dot-product attention available (what the reference runs on an H100 with torch 2.x).  DESIGN section 7.
+LG_PRUNE_MIN_POINTS = 1536
+
+
+class _LighterGlue:
+    """`XFeat.lighterglue`: the matcher's handle (packed weights on the device, xfeat_lg_create)."""
+
+    def __init__(self, owner: "XFeat", weights):
+        self._lib = owner._lib
+        blob = _weights.pack_lighterglue(_weights.load_lighterglue_state(weights))
+        handle = ctypes.c_void_p()
+        _lib.check(self._lib.xfeat_lg_create(ctypes.byref(handle), owner.dev.index, blob.ctypes.data, blob.size), "xfeat_lg_create")
+        self.ctx = handle
+
+    def __del__(self):
+        try:
+            if getattr(self, "ctx", None):
+                self._lib.xfeat_lg_destroy(self.ctx)
+                self.ctx = None
+        except Exception:
+            pass
+
+
 class XFeat(torch.nn.Module):
     """H100-native XFeat inference (sparse `detectAndCompute` / `match_xfeat`, semi-dense `match_xfeat_star`)."""
 
     def __init__(self, weights=_weights.DEFAULT_WEIGHTS, top_k: int = 4096, detection_threshold: float = 0.05,
-                 device: Optional[int] = None):
-        # reference: xfeat.py:23-46.  `weights`: path (.pt/.npz), state_dict mapping, or None (random init)
+                 device: Optional[int] = None, lighterglue_weights=_weights.LG_DEFAULT_WEIGHTS):
+        # reference: xfeat.py:23-46.  `weights`: path (.pt/.npz), state_dict mapping, or None (random init).
+        # `lighterglue_weights`: the published xfeat-lighterglue.pt (or its matcher state re-saved as .npz, or a mapping); read on
+        # the first LighterGlue call
         super().__init__()
         if not torch.cuda.is_available():
             raise RuntimeError("accelerated_features_b200.XFeat needs a CUDA device (sm_90a); there is no CPU fallback")
@@ -132,6 +159,7 @@ class XFeat(torch.nn.Module):
         self.interpolator = InterpolateSparse2d("bicubic")   # xfeat.py:37
         self.kornia_available = False
         self.lighterglue = None
+        self._lighterglue_weights = lighterglue_weights
         self._pipe = None                               # lazily built copy pipeline of match_xfeat_stream
 
     def __del__(self):
@@ -716,10 +744,94 @@ class XFeat(torch.nn.Module):
         out = [matches[b, :n[b]] for b in range(len(n))]
         return out if len(n) > 1 else (out[0][:, :2].cpu().numpy(), out[0][:, 2:].cpu().numpy())
 
+    # ------------------------------------------------------------------------------------------------------------
+    # LighterGlue matching (csrc/lighterglue.cu)
+    # ------------------------------------------------------------------------------------------------------------
+    def _lg(self) -> "_LighterGlue":
+        if self.lighterglue is None:                    # loaded on first use, as the reference does (xfeat.py:143-145)
+            self.lighterglue = _LighterGlue(self, self._lighterglue_weights)
+        return self.lighterglue
+
     @torch.inference_mode()
-    def match_lighterglue(self, d0, d1, min_conf=0.1):
-        # reference: xfeat.py:131-162 -- needs kornia's LightGlue, which is outside this hot path (SURVEY section 2, #8)
-        raise RuntimeError('We rely on kornia for LightGlue. Install with: pip install kornia')
+    def match_lighterglue_batch(self, kpts0, desc0, n0, size0, kpts1, desc1, n1, size1, min_conf: float = 0.1,
+                                prune_min_points: Optional[int] = LG_PRUNE_MIN_POINTS):
+        """LighterGlue on B pairs of fixed-capacity device inputs, no host sync.  kpts (B,n_max,2) pixel (x,y), desc (B,n_max,64),
+        n (B) int32 point counts, size (B,2) image size (W,H); the two sides share n_max.  `prune_min_points`: an image with more
+        points than this is pruned after layers 0..4 (LightGlue's point pruning, width_confidence 0.95); None disables pruning.
+        Returns device tensors idx0 (ascending), idx1 (B,n_max) int64, scores (B,n_max), n_matches (B) int32."""
+        lg = self._lg()
+        t = lambda x, dt: x.to(self.dev, dt).contiguous()       # noqa: E731
+        kpts0, kpts1, desc0, desc1 = (t(x, torch.float32) for x in (kpts0, kpts1, desc0, desc1))
+        size0, size1 = t(torch.as_tensor(size0), torch.float32), t(torch.as_tensor(size1), torch.float32)
+        n0, n1 = t(torch.as_tensor(n0), torch.int32), t(torch.as_tensor(n1), torch.int32)
+        B, n_max = kpts0.shape[:2]
+        if (kpts1.shape != (B, n_max, 2) or kpts0.shape != (B, n_max, 2) or desc0.shape != (B, n_max, 64)
+                or desc1.shape != (B, n_max, 64) or size0.shape != (B, 2) or size1.shape != (B, 2)
+                or n0.shape != (B,) or n1.shape != (B,)):
+            raise RuntimeError("match_lighterglue_batch: kpts (B,n_max,2), desc (B,n_max,64), n (B), size (B,2) on both sides")
+        idx0 = self._empty((B, n_max), torch.int64)
+        idx1 = self._empty((B, n_max), torch.int64)
+        scores = self._empty((B, n_max))
+        cnt = self._empty((B,), torch.int32)
+        ws = self._workspace(self._lib.xfeat_lg_workspace_bytes(B, n_max))
+        T = -1 if prune_min_points is None else int(prune_min_points)
+        with torch.cuda.device(self.dev):
+            _lib.check(self._lib.xfeat_lg_match(lg.ctx, B, n_max, kpts0.data_ptr(), desc0.data_ptr(), n0.data_ptr(), size0.data_ptr(),
+                                                kpts1.data_ptr(), desc1.data_ptr(), n1.data_ptr(), size1.data_ptr(), float(min_conf),
+                                                T, idx0.data_ptr(), idx1.data_ptr(), scores.data_ptr(), cnt.data_ptr(),
+                                                ws.data_ptr(), ws.numel(), self._stream()), "xfeat_lg_match")
+        return idx0, idx1, scores, cnt
+
+    @torch.inference_mode()
+    def match_lighterglue(self, d0, d1, min_conf=0.1, prune_min_points: Optional[int] = LG_PRUNE_MIN_POINTS):
+        """Match XFeat sparse features with LighterGlue (reference: xfeat.py:131-162).
+        d0, d1: dicts with 'keypoints' (N,2), 'descriptors' (N,64), 'image_size' (W,H).
+        Returns mkpts_0, mkpts_1 (N,2) and idx (N,2) int64 as np.ndarray."""
+        k0, k1 = d0["keypoints"].to(self.dev).float(), d1["keypoints"].to(self.dev).float()
+        n0, n1 = len(k0), len(k1)
+        n_max = max(n0, n1, 1)
+
+        def pad(x, n, c):
+            out = torch.zeros((1, n_max, c), dtype=torch.float32, device=self.dev)
+            out[0, :n] = x.to(self.dev).float().reshape(n, c)
+            return out
+        idx0, idx1, _, cnt = self.match_lighterglue_batch(
+            pad(k0, n0, 2), pad(d0["descriptors"], n0, 64), torch.tensor([n0]), torch.tensor([list(d0["image_size"])]),
+            pad(k1, n1, 2), pad(d1["descriptors"], n1, 64), torch.tensor([n1]), torch.tensor([list(d1["image_size"])]),
+            min_conf, prune_min_points)
+        n = int(cnt.item())
+        i0, i1 = idx0[0, :n], idx1[0, :n]
+        return k0[i0].cpu().numpy(), k1[i1].cpu().numpy(), torch.stack([i0, i1], -1).cpu().numpy()
+
+    @torch.inference_mode()
+    def match_xfeat_lighterglue_batch(self, imgs1, imgs2, top_k=None, min_conf: float = 0.1,
+                                      prune_min_points: Optional[int] = LG_PRUNE_MIN_POINTS) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+        """detectAndCompute on both image sets, LighterGlue on every pair b = (imgs1[b], imgs2[b]) and the keypoint gather, all
+        on the device with one host synchronisation.  Returns per pair (mkpts_0, mkpts_1, idx (N,2)) as match_lighterglue does."""
+        if top_k is None: top_k = self.top_k
+        x1, da = self._parse_input(imgs1)
+        x2, db = self._parse_input(imgs2)
+        x1, x2 = self._to_bchw(x1), self._to_bchw(x2)
+        B = x1.shape[0]
+        if x2.shape[0] != B:
+            raise RuntimeError("the two image sets must have the same batch size")
+        if x1.shape[1:] == x2.shape[1:]:
+            o = self._detect_sparse_device([x1, x2], top_k, self.detection_threshold, [da, db])
+            k0, k1, d0, d1 = o["keypoints"][:B], o["keypoints"][B:], o["descriptors"][:B], o["descriptors"][B:]
+            n0, n1 = o["n_valid"][:B], o["n_valid"][B:]
+        else:
+            o1 = self._detect_sparse_device(x1, top_k, self.detection_threshold, da)
+            o2 = self._detect_sparse_device(x2, top_k, self.detection_threshold, db)
+            k0, k1, d0, d1, n0, n1 = (o1["keypoints"], o2["keypoints"], o1["descriptors"], o2["descriptors"], o1["n_valid"],
+                                      o2["n_valid"])
+        size0 = torch.tensor([[x1.shape[3], x1.shape[2]]] * B, dtype=torch.float32)
+        size1 = torch.tensor([[x2.shape[3], x2.shape[2]]] * B, dtype=torch.float32)
+        idx0, idx1, _, cnt = self.match_lighterglue_batch(k0, d0, n0, size0, k1, d1, n1, size1, min_conf, prune_min_points)
+        mk0, mk1, cnt = self._gather_matches(k0, k1, idx0, idx1, cnt, B, top_k)
+        c = cnt.tolist()                                              # the only host sync
+        self._check_counts(c, "match_xfeat_lighterglue_batch")
+        mk0, mk1, i0, i1 = (t.cpu().numpy() for t in (mk0, mk1, idx0, idx1))
+        return [(mk0[b, :c[b]], mk1[b, :c[b]], np.stack([i0[b, :c[b]], i1[b, :c[b]]], -1)) for b in range(B)]
 
     # ------------------------------------------------------------------------------------------------------------
     # the reference's helper methods, each through its own kernel of the library

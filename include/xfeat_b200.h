@@ -259,6 +259,42 @@ XF_API int xfeat_ransac_essential(const float* d_x0, const float* d_x1, const in
                                   int iters, uint32_t seed, float* d_E, uint8_t* d_inliers, int32_t* d_n_inliers, void* d_ws,
                                   size_t ws_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * LighterGlue matcher (csrc/lighterglue.cu; fp32 CUDA-core kernels), its own handle and weight blob
+ * ------------------------------------------------------------------------------------------------------- */
+typedef struct xfeat_lg_ctx xfeat_lg_ctx;
+
+/* Number of floats of the packed LighterGlue blob (accelerated_features_b200/weights.py pack_lighterglue). */
+XF_API size_t xfeat_lg_packed_weight_floats(void);
+/* replaces: LighterGlue() (modules/lighterglue.py:29-49).  `packed_host` is a HOST pointer. */
+XF_API int xfeat_lg_create(xfeat_lg_ctx** out, int device, const float* packed_host, size_t n_floats);
+XF_API void xfeat_lg_destroy(xfeat_lg_ctx* ctx);
+XF_API size_t xfeat_lg_workspace_bytes(int batch, int n_max);
+/* replaces: XFeat.match_lighterglue (xfeat.py:131-162) -> LighterGlue.forward (lighterglue.py:51-57) for a batch of pairs.
+ * Inputs per side s = 0, 1: d_kpts (batch, n_max, 2) pixel (x, y), d_desc (batch, n_max, 64), d_n (batch) int32 device counts
+ * (XF_N_OVERFLOW gives d_n_matches = XF_N_OVERFLOW), d_size (batch, 2) fp32 image size (W, H).
+ * prune_min_points >= 0: after layers 0..4 an image with more points than this keeps only those with sigmoid(matchability) >
+ * 0.05; < 0: no pruning.  Outputs at capacity n_max: d_idx0 (ascending) / d_idx1 (batch, n_max) int64 indices into the inputs,
+ * d_scores (batch, n_max) = exp(log-assignment row maximum), d_n_matches (batch).  Mutual arg-max (first index on ties) with
+ * score > min_conf.  No host synchronisation: the counts after pruning stay on the device. */
+XF_API int xfeat_lg_match(xfeat_lg_ctx* ctx, int batch, int n_max, const float* d_kpts0, const float* d_desc0,
+                          const int32_t* d_n0, const float* d_size0, const float* d_kpts1, const float* d_desc1,
+                          const int32_t* d_n1, const float* d_size1, float min_conf, int prune_min_points, int64_t* d_idx0,
+                          int64_t* d_idx1, float* d_scores, int32_t* d_n_matches, void* d_ws, size_t ws_bytes, void* stream);
+/* Test hook: xfeat_lg_match's inputs, stopped after `n_layers` (0..6) layers.  Image g = s * batch + b.  Outputs:
+ * d_x (2, batch, n_max, 96) the descriptors of the surviving points, compacted; d_ind (2, batch, n_max) int32 their input
+ * indices; d_cnt (2, batch) int32 their counts; with n_layers == 6 optionally (both or neither) d_best (2, batch, n_max) fp32 the
+ * log-assignment row (s = 0) / column (s = 1) maximum and d_arg its first arg-max (int32, index among the surviving points). */
+XF_API int xfeat_lg_debug(xfeat_lg_ctx* ctx, int batch, int n_max, const float* d_kpts0, const float* d_desc0, const int32_t* d_n0,
+                          const float* d_size0, const float* d_kpts1, const float* d_desc1, const int32_t* d_n1,
+                          const float* d_size1, int prune_min_points, int n_layers, float* d_x, int32_t* d_ind, int32_t* d_cnt,
+                          float* d_best, int32_t* d_arg, void* d_ws, size_t ws_bytes, void* stream);
+/* Test hook: the attention kernel alone.  d_q / d_k / d_v (groups, n_max, ld) rows (96 values each from the pointer), d_n (groups)
+ * int32 counts; cross == 0: group g attends to its own keys, 1: to those of group (g + groups/2) mod groups.
+ * d_out (groups, n_max, 96) = softmax(q k^T / sqrt(96)) v for the rows below the count. */
+XF_API int xfeat_lg_debug_attention(const float* d_q, const float* d_k, const float* d_v, int ld, const int32_t* d_n, int groups,
+                                    int n_max, int cross, float* d_out, void* stream);
+
 /* Test hook: run one folded conv layer of the packed table (index into csrc/layers.h) through the generic
  * kernels. in (B,Hi,Wi,Cin) NHWC -> out (B,Ho,Wo,Cout). */
 XF_API int xfeat_debug_conv_layer(xfeat_ctx* ctx, int layer, const float* d_in, int B, int Hi, int Wi, float* d_out,
