@@ -152,6 +152,12 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
     tc::mbar_wait(w_full, 0);
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      // one wgmma group per stage, and (with >= 3 stages) one group left in flight across stages: the wait after issuing stage t
+      // retires stage t-1, whose buffer goes back to the producer, and the tensor pipe drains only at the end of the tile.  With
+      // 2 stages each stage drains before the next is awaited: releasing t-1 only once t has arrived would leave a single
+      // operand load in flight.
+      constexpr int INFLIGHT = C::NS > 2 ? 1 : 0;
+      int s_prev = 0;
       for (int tap0 = 0; tap0 < C::TAPS; tap0 += C::TPS, ++it) {
         const int s = it % C::NS;
         tc::mbar_wait(&a_full[s], (it / C::NS) & 1);
@@ -190,52 +196,69 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
           }
         }
         tc::wgmma_commit();
+        tc::wgmma_wait<INFLIGHT>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        if (INFLIGHT == 0 || tap0 > 0) {
+          __syncwarp();
+          if (lane == 0) tc::mbar_arrive(&a_empty[INFLIGHT ? s_prev : s]);   // this warp's reads of that stage are complete
+        }
+        s_prev = s;
+      }
+      if (INFLIGHT) {
         tc::wgmma_wait<0>();
         tc::acc_fence(acc0);
         tc::acc_fence(acc1);
         __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&a_empty[s]);   // this warp's reads of the stage are complete
+        if (lane == 0) tc::mbar_arrive(&a_empty[s_prev]);
       }
       // ---------------- epilogue ----------------
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      uint32_t v[N2];
+      const bool store = y < P.H && x < P.W;
+      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
+      float skipv = 0.f;
+      if (store && P.skip_xn != nullptr) {
+        // AvgPool2d(4,4) of the normalised gray image, then 1x1 conv 1 -> 24 with bias, added AFTER the ReLU (model.py:140)
+        const int W0 = P.W * 4;
+        const float* xp = P.skip_xn + ((int64_t)b * P.H * 4 + y * 4) * W0 + x * 4;
+        float sacc = 0.f;
 #pragma unroll
-      for (int c = 0; c < N2 / 32; ++c) {
-        uint32_t t[32];
-        tc::acc_rows<32>(sStg, acc0, acc1, c * 32, r, 1, t);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[c * 32 + j] = t[j];
+        for (int rr = 0; rr < 4; ++rr) {
+          const float4 t = __ldg(reinterpret_cast<const float4*>(xp + (int64_t)rr * W0));
+          sacc += t.x; sacc += t.y; sacc += t.z; sacc += t.w;
+        }
+        skipv = sacc * (1.0f / 16.0f);
       }
-      if (y < P.H && x < P.W) {
-        const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-        float o[NOUT];
+      // 32 output channels at a time: the group-0 columns c and the group-1 columns NOUT + c of the same channels, so that no
+      // copy of all 2 * NOUT accumulator columns sits next to the accumulators
 #pragma unroll
-        for (int c = 0; c < NOUT; ++c) {
-          float t0 = fmaf(__uint_as_float(v[c]) + __uint_as_float(v[NOUT + c]), P.inv_wscale, sBias[c]);
-          if (P.relu) t0 = fmaxf(t0, 0.f);
-          o[c] = t0;
-        }
-        if (P.skip_xn != nullptr) {
-          // AvgPool2d(4,4) of the normalised gray image, then 1x1 conv 1 -> 24 with bias, added AFTER the ReLU (model.py:140)
-          const int W0 = P.W * 4;
-          const float* xp = P.skip_xn + ((int64_t)b * P.H * 4 + y * 4) * W0 + x * 4;
-          float sacc = 0.f;
+      for (int c0 = 0; c0 < NOUT; c0 += 32) {
+        uint32_t vh[32];
+        tc::acc_rows<32>(sStg, acc0, acc1, c0, r, 1, vh);
+        float a[32];   // group-0 + group-1 columns of channels c0..c0+31
 #pragma unroll
-          for (int rr = 0; rr < 4; ++rr) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(xp + (int64_t)rr * W0));
-            sacc += t.x; sacc += t.y; sacc += t.z; sacc += t.w;
+        for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
+        tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, r, 1, a);
+        if (store) {
+          float o[32];
+#pragma unroll
+          for (int c = 0; c < 32; ++c) {
+            float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
+            if (P.relu) t0 = fmaxf(t0, 0.f);
+            o[c] = t0;
           }
-          const float skipv = sacc * (1.0f / 16.0f);
+          if (P.skip_xn != nullptr) {
 #pragma unroll
-          for (int c = 0; c < NOUT; ++c) o[c] += fmaf(skipv, sSkip[c], sSkip[NOUT + c]);
-        }
-        if (P.out_f32) tc::store_f32_row<NOUT>(P.out_f32 + pix * P.f32_c + P.f32_co0, o, P.n_real);
-        if (P.out_split) {
-          // [hi(split_c) | lo(split_c)]; this N tile owns channels f32_co0 .. f32_co0+NOUT-1 (padded channels: exact zeros)
-          __half* hp = P.out_split + pix * (2 * P.split_c) + P.f32_co0;
-          tc::store_split_row<NOUT>(hp, hp + P.split_c, o);
+            for (int c = 0; c < 32; ++c) o[c] += fmaf(skipv, sSkip[c0 + c], sSkip[NOUT + c0 + c]);
+          }
+          if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + P.f32_co0 + c0, o, P.n_real - c0);
+          if (P.out_split) {
+            // [hi(split_c) | lo(split_c)]; this N tile owns channels f32_co0 .. f32_co0+NOUT-1 (padded channels: exact zeros)
+            __half* hp = P.out_split + pix * (2 * P.split_c) + P.f32_co0 + c0;
+            tc::store_split_row<32>(hp, hp + P.split_c, o);
+          }
         }
       }
     }
@@ -333,7 +356,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
           }
         }
         tc::wgmma_commit();
-        tc::wgmma_wait<0>();
+        tc::wgmma_wait<0>();   // two stages: drain per tap (see conv_tc_kernel)
         tc::acc_fence(acc0);
         tc::acc_fence(acc1);
         __syncwarp();
@@ -342,25 +365,29 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      uint32_t v0[32], v1[32], v2[32], v3[32];
-      tc::acc_rows<32>(sStg, acc0, acc1, 0, r, 1, v0);
-      tc::acc_rows<32>(sStg, acc0, acc1, 32, r, 1, v1);
-      tc::acc_rows<32>(sStg, acc0, acc1, 64, r, 1, v2);
-      tc::acc_rows<32>(sStg, acc0, acc1, 96, r, 1, v3);
-      if (y < P.H && x < P.W) {
-        const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-        float o[NOUT];
+      const bool store = y < P.H && x < P.W;
+      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          float t0 = fmaf(__uint_as_float(v0[c]) + __uint_as_float(v2[c]), P.inv_wscale, sBias[c]);
-          float t1 = fmaf(__uint_as_float(v1[c]) + __uint_as_float(v3[c]), P.inv_wscale, sBias[32 + c]);
-          if (P.relu) { t0 = fmaxf(t0, 0.f); t1 = fmaxf(t1, 0.f); }
-          o[c] = t0; o[32 + c] = t1;
-        }
-        if (P.out_f32) tc::store_f32_row<NOUT>(P.out_f32 + pix * P.f32_c + co0, o, NOUT);
-        if (P.out_split) {
-          __half* hp = P.out_split + pix * (2 * P.split_c) + co0;
-          tc::store_split_row<NOUT>(hp, hp + P.split_c, o);
+      for (int c0 = 0; c0 < NOUT; c0 += 32) {   // 32 channels at a time: group-0 columns c0.., group-1 columns NOUT + c0..
+        uint32_t vh[32];
+        tc::acc_rows<32>(sStg, acc0, acc1, c0, r, 1, vh);
+        float a[32];   // group-0 + group-1 columns of channels c0..c0+31
+#pragma unroll
+        for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
+        tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, r, 1, a);
+        if (store) {
+          float o[32];
+#pragma unroll
+          for (int c = 0; c < 32; ++c) {
+            float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
+            if (P.relu) t0 = fmaxf(t0, 0.f);
+            o[c] = t0;
+          }
+          if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + co0 + c0, o, 32);
+          if (P.out_split) {
+            __half* hp = P.out_split + pix * (2 * P.split_c) + co0 + c0;
+            tc::store_split_row<32>(hp, hp + P.split_c, o);
+          }
         }
       }
     }

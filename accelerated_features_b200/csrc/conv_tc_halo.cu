@@ -152,12 +152,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
             tc::wgmma_f16<N2>(acc1, ahi1 + 2 * k, wboth + 2 * k, (tap | k) ? 1u : 0u);
           }
         }
-        tc::wgmma_commit();
-        tc::wgmma_wait<0>();
-        tc::acc_fence(acc0);
-        tc::acc_fence(acc1);
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&p_empty[s_hi]);   // hi patch buffer may be refilled
+        tc::wgmma_commit();   // the hi group stays in flight while the lo patch is awaited and the lo MMAs are queued
         tc::mbar_wait(&p_full[s_lo], (li_lo / NP) & 1);
         tc::wgmma_fence();
         for (int tap = 0; tap < 9; ++tap) {
@@ -172,6 +167,11 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
           }
         }
         tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) tc::mbar_arrive(&p_empty[s_hi]);   // hi group retired: the hi patch buffer may be refilled
         tc::wgmma_wait<0>();
         tc::acc_fence(acc0);
         tc::acc_fence(acc1);
@@ -182,6 +182,9 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
         const uint32_t p_base = tc::smem_u32(sP) + (uint32_t)s * PB;
         tc::mbar_wait(&p_full[s], (tcount / NP) & 1);
         tc::wgmma_fence();
+        // unrolled: the scale-d flags become constants.  Left as a loop, ptxas (C7520) serialises every wgmma of this path
+        // behind a warpgroup.arrive + wait of its own.
+#pragma unroll
         for (int tap = 0; tap < 9; ++tap) {
           const uint32_t shift = (uint32_t)((tap / 3) * P.PW + (tap % 3)) * (uint32_t)ROWB;
           const uint64_t a0 = make_desc_rows_at<ROWB>(p_base + shift, P.desc_mode);
@@ -212,31 +215,50 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
       const int y = ty_ * P.TH + mh, x = tx_ * P.TW + mw;
-      uint32_t v[N2];
+      const bool store = lane_ok && y < P.H && x < P.W;
+      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
       if constexpr (NOUT == 8) {
+        uint32_t v[N2];
         tc::acc_rows<16>(sStg, acc0, acc1, 0, m, 1, v);
+        if (store) {
+          float o[NOUT];
+#pragma unroll
+          for (int c = 0; c < NOUT; ++c) {
+            float t0 = fmaf(__uint_as_float(v[c]) + __uint_as_float(v[NOUT + c]), P.inv_wscale, sBias[c]);
+            if (P.relu) t0 = fmaxf(t0, 0.f);
+            o[c] = t0;
+          }
+          if (P.out_f32) tc::store_f32_row<NOUT>(P.out_f32 + pix * P.f32_c, o, P.n_real);
+          if (P.out_split) {
+            __half* hp = P.out_split + pix * (2 * NOUT);
+            tc::store_split_row<NOUT>(hp, hp + NOUT, o);
+          }
+        }
       } else {
+        // 32 output channels at a time: the group-0 columns c and the group-1 columns NOUT + c of the same channels, so that
+        // no copy of all 2 * NOUT accumulator columns sits next to the accumulators
 #pragma unroll
-        for (int c = 0; c < N2 / 32; ++c) {
-          uint32_t t[32];
-          tc::acc_rows<32>(sStg, acc0, acc1, c * 32, m, 1, t);
+        for (int c0 = 0; c0 < NOUT; c0 += 32) {
+          uint32_t vh[32];
+          tc::acc_rows<32>(sStg, acc0, acc1, c0, m, 1, vh);
+          float a[32];   // group-0 + group-1 columns of channels c0..c0+31
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[c * 32 + j] = t[j];
-        }
-      }
-      if (lane_ok && y < P.H && x < P.W) {
-        const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-        float o[NOUT];
+          for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
+          tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, m, 1, a);
+          if (store) {
+            float o[32];
 #pragma unroll
-        for (int c = 0; c < NOUT; ++c) {
-          float t0 = fmaf(__uint_as_float(v[c]) + __uint_as_float(v[NOUT + c]), P.inv_wscale, sBias[c]);
-          if (P.relu) t0 = fmaxf(t0, 0.f);
-          o[c] = t0;
-        }
-        if (P.out_f32) tc::store_f32_row<NOUT>(P.out_f32 + pix * P.f32_c, o, P.n_real);
-        if (P.out_split) {
-          __half* hp = P.out_split + pix * (2 * NOUT);
-          tc::store_split_row<NOUT>(hp, hp + NOUT, o);
+            for (int c = 0; c < 32; ++c) {
+              float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
+              if (P.relu) t0 = fmaxf(t0, 0.f);
+              o[c] = t0;
+            }
+            if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + c0, o, P.n_real - c0);
+            if (P.out_split) {
+              __half* hp = P.out_split + pix * (2 * NOUT) + c0;
+              tc::store_split_row<32>(hp, hp + NOUT, o);
+            }
+          }
         }
       }
     }

@@ -208,6 +208,20 @@ __device__ __forceinline__ void acc_rows(float* stg, const float (&d0)[R], const
   stage_read<CW>(stg, wt, v);
   wg_sync(bar);
 }
+// a[j] += column c0 + j of row `wt`: the split-term epilogues sum the group-0 and group-1 columns of a channel without holding
+// both 32-column chunks in registers at once
+template <int CW, int R>
+__device__ __forceinline__ void acc_rows_add(float* stg, const float (&d0)[R], const float (&d1)[R], int c0, int wt, int bar,
+                                             float (&a)[CW]) {
+  stage_write<CW>(stg, d0, d1, c0, wt);
+  wg_sync(bar);
+#pragma unroll
+  for (int k = 0; k < CW / 4; ++k) {
+    const float4 t = *reinterpret_cast<const float4*>(stg + stg_off(wt, 4 * k));
+    a[4 * k] += t.x; a[4 * k + 1] += t.y; a[4 * k + 2] += t.z; a[4 * k + 3] += t.w;
+  }
+  wg_sync(bar);
+}
 
 // ---------------------------------------------------------------- epilogue stores
 // 32 bytes per thread and call as two 16-byte stores: the conv epilogues write one pixel row per thread, so a warp-wide store
