@@ -13,9 +13,9 @@
 //   * the A operand of tap (dy,dx) is the input patch shifted by (dy-1, dx-1): ONE 4-D TMA box {64 ch, TW, TH, 1} per
 //     term, 128B-swizzled K-major, out-of-image coordinates zero-filled by the TMA unit (= the conv's zero padding);
 //   * the folded, pre-split weights of all taps stay resident in shared memory for the life of the (persistent) CTA;
-//   * warps 0-3 = one warpgroup that issues the wgmmas (two 64-row slabs per tile) and runs the epilogue, one pixel row per
-//     thread (the accumulator fragments are handed over through a 16 KB staging buffer); warp 4 = TMA producer, which runs
-//     up to NS taps ahead, so the operand loads of tile i+1 overlap the epilogue of tile i.
+//   * warps 0-3 = one warpgroup that issues the wgmmas (two 64-row slabs per tile) and runs the epilogue, which writes the
+//     outputs from the accumulator fragments into a 16 KB staging region and stores them as TMA boxes (tc::conv_epilogue);
+//     warp 4 = TMA producer, which runs up to NS taps ahead, so the operand loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda_fp16.h>
 
 #include <vector>
@@ -66,10 +66,11 @@ struct ConvTcParams {
   int stride;         // 1 or 2
   int pad;            // KS / 2
   int tw_log2;        // TW = 1 << tw_log2, TH = 128 / TW
-  __half* out_split;  // (B,H,W,2*split_c) [hi(split_c) | lo(split_c)] or null; split_c = 32 or 64
+  CUtensorMap smap;   // split output (B,H,W,2*split_c) [hi(split_c) | lo(split_c)], split_c = 32 or 64; box {32, TW, TH, 1}
+  CUtensorMap fmap;   // fp32 output (B,H,W,f32_c); box {16, TW, TH, 1}
+  int has_split, has_f32;
   int split_c;
-  float* out_f32;     // (B,H,W,f32_c) or null; this CTA's channels start at f32_co0, n_real of them are real
-  int f32_c, f32_co0, n_real;
+  int f32_co0, n_real;   // this CTA's first output channel; n_real of its NOUT channels are real
   int relu;
   // optional skip branch of the stem (model.py:40-41,140): out += avgpool4(xn) * skip_w + skip_b, xn = (B, 4H, 4W) fp32
   const float* skip_xn;
@@ -84,7 +85,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sW = base;
   unsigned char* sA = base + C::W_BYTES;
-  float* sStg = reinterpret_cast<float*>(base + C::W_BYTES + C::A_BYTES);
+  unsigned char* sStg = base + C::W_BYTES + C::A_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + C::A_BYTES + tc::STG_BYTES);
   uint64_t* w_full = bars;
   uint64_t* a_full = bars + 1;                 // [NS]
@@ -99,6 +100,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
 
   if (threadIdx.x < NOUT) sBias[threadIdx.x] = (threadIdx.x < P.n_real) ? __ldg(P.bias + threadIdx.x) : 0.f;
   float* sSkip = sBias + NOUT;   // [2][NOUT]: skip weights, skip biases (zero when unused / padded)
+  float* sSkipv = sSkip + 2 * NOUT;   // [128]: pooled skip input per tile pixel
   if (threadIdx.x < 2 * NOUT) {
     const int c = threadIdx.x % NOUT, wb = threadIdx.x / NOUT;
     sSkip[threadIdx.x] = (P.skip_w != nullptr && c < 24) ? __ldg(P.skip_w + wb * 24 + c) : 0.f;
@@ -106,6 +108,8 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
   if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
+    if (P.has_split) tc::tma_prefetch_desc(&P.smap);
+    if (P.has_f32) tc::tma_prefetch_desc(&P.fmap);
     tc::mbar_init(w_full, 1);
     for (int i = 0; i < C::NS; ++i) {
       tc::mbar_init(&a_full[i], 1);
@@ -149,6 +153,20 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
     const int r = threadIdx.x;
     const int ph_ = r >> P.tw_log2, pw_ = r & (TW - 1);
     float acc0[NOUT], acc1[NOUT];                    // rows 0-63 / 64-127, N2 columns each
+    int srow[4];                                     // staging row = GEMM row = pixel of the TW x TH tile
+#pragma unroll
+    for (int h = 0; h < 4; ++h) srow[h] = tc::frag_row(r, h);
+    tc::ConvEpi E;
+    E.split = P.has_split ? &P.smap : nullptr;
+    E.f32 = P.has_f32 ? &P.fmap : nullptr;
+    E.split_c = P.split_c;
+    E.co = P.f32_co0;
+    E.inv_wscale = P.inv_wscale;
+    E.relu = P.relu;
+    E.bias = sBias;
+    E.skip_w = P.skip_xn != nullptr ? sSkip : nullptr;
+    E.skip_v = sSkipv;
+    uint32_t piece = 0;
     tc::mbar_wait(w_full, 0);
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -215,53 +233,32 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc_kernel(const __grid_con
       // ---------------- epilogue ----------------
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
-      const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      const bool store = y < P.H && x < P.W;
-      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-      float skipv = 0.f;
-      if (store && P.skip_xn != nullptr) {
-        // AvgPool2d(4,4) of the normalised gray image, then 1x1 conv 1 -> 24 with bias, added AFTER the ReLU (model.py:140)
-        const int W0 = P.W * 4;
-        const float* xp = P.skip_xn + ((int64_t)b * P.H * 4 + y * 4) * W0 + x * 4;
-        float sacc = 0.f;
+      E.x0 = tx_ * TW;
+      E.y0 = ty_ * TH;
+      E.b = b;
+      if (P.skip_xn != nullptr) {
+        // AvgPool2d(4,4) of the normalised gray image, one tile pixel per thread; the 1x1 conv 1 -> 24 with bias is added AFTER
+        // the ReLU (model.py:140)
+        const int y = E.y0 + ph_, x = E.x0 + pw_;
+        float skipv = 0.f;
+        if (y < P.H && x < P.W) {
+          const int W0 = P.W * 4;
+          const float* xp = P.skip_xn + ((int64_t)b * P.H * 4 + y * 4) * W0 + x * 4;
+          float sacc = 0.f;
 #pragma unroll
-        for (int rr = 0; rr < 4; ++rr) {
-          const float4 t = __ldg(reinterpret_cast<const float4*>(xp + (int64_t)rr * W0));
-          sacc += t.x; sacc += t.y; sacc += t.z; sacc += t.w;
+          for (int rr = 0; rr < 4; ++rr) {
+            const float4 t = __ldg(reinterpret_cast<const float4*>(xp + (int64_t)rr * W0));
+            sacc += t.x; sacc += t.y; sacc += t.z; sacc += t.w;
+          }
+          skipv = sacc * (1.0f / 16.0f);
         }
-        skipv = sacc * (1.0f / 16.0f);
+        sSkipv[r] = skipv;
+        tc::wg_sync(1);
       }
-      // 32 output channels at a time: the group-0 columns c and the group-1 columns NOUT + c of the same channels, so that no
-      // copy of all 2 * NOUT accumulator columns sits next to the accumulators
-#pragma unroll
-      for (int c0 = 0; c0 < NOUT; c0 += 32) {
-        uint32_t vh[32];
-        tc::acc_rows<32>(sStg, acc0, acc1, c0, r, 1, vh);
-        float a[32];   // group-0 + group-1 columns of channels c0..c0+31
-#pragma unroll
-        for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
-        tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, r, 1, a);
-        if (store) {
-          float o[32];
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
-            if (P.relu) t0 = fmaxf(t0, 0.f);
-            o[c] = t0;
-          }
-          if (P.skip_xn != nullptr) {
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] += fmaf(skipv, sSkip[c0 + c], sSkip[NOUT + c0 + c]);
-          }
-          if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + P.f32_co0 + c0, o, P.n_real - c0);
-          if (P.out_split) {
-            // [hi(split_c) | lo(split_c)]; this N tile owns channels f32_co0 .. f32_co0+NOUT-1 (padded channels: exact zeros)
-            __half* hp = P.out_split + pix * (2 * P.split_c) + P.f32_co0 + c0;
-            tc::store_split_row<32>(hp, hp + P.split_c, o);
-          }
-        }
-      }
+      // this N tile owns output channels f32_co0 .. f32_co0+NOUT-1 (padded split channels: exact zeros)
+      tc::conv_epilogue<NOUT>(acc0, acc1, sStg, piece, srow, E);
     }
+    if (threadIdx.x == 0) tc::bulk_wait_all();
   }
 }
 
@@ -280,7 +277,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sS = base;
-  float* sStg = reinterpret_cast<float*>(base + NS * (size_t)C128_STAGE);
+  unsigned char* sStg = base + NS * (size_t)C128_STAGE;
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + NS * (size_t)C128_STAGE + tc::STG_BYTES);
   uint64_t* s_full = bars;           // [NS]
   uint64_t* s_empty = bars + NS;     // [NS]
@@ -298,6 +295,8 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
   if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
+    if (P.has_split) tc::tma_prefetch_desc(&P.smap);
+    if (P.has_f32) tc::tma_prefetch_desc(&P.fmap);
     for (int i = 0; i < NS; ++i) {
       tc::mbar_init(&s_full[i], 1);
       tc::mbar_init(&s_empty[i], 4);
@@ -331,8 +330,21 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
   } else {
     constexpr uint32_t HALF = (64 * 128) >> 4;   // descriptor offset of rows 64-127
     const int r = threadIdx.x;
-    const int ph_ = r >> P.tw_log2, pw_ = r & (TW - 1);
     float acc0[NOUT], acc1[NOUT];                 // rows 0-63 / 64-127, 2*NOUT columns each
+    int srow[4];
+#pragma unroll
+    for (int h = 0; h < 4; ++h) srow[h] = tc::frag_row(r, h);
+    tc::ConvEpi E;
+    E.split = P.has_split ? &P.smap : nullptr;
+    E.f32 = P.has_f32 ? &P.fmap : nullptr;
+    E.split_c = P.split_c;
+    E.co = co0;
+    E.inv_wscale = P.inv_wscale;
+    E.relu = P.relu;
+    E.bias = sBias;
+    E.skip_w = nullptr;
+    E.skip_v = nullptr;
+    uint32_t piece = 0;
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
       for (int tap = 0; tap < TAPS; ++tap, ++it) {
@@ -364,33 +376,12 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
       }
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
-      const int y = ty_ * TH + ph_, x = tx_ * TW + pw_;
-      const bool store = y < P.H && x < P.W;
-      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-#pragma unroll
-      for (int c0 = 0; c0 < NOUT; c0 += 32) {   // 32 channels at a time: group-0 columns c0.., group-1 columns NOUT + c0..
-        uint32_t vh[32];
-        tc::acc_rows<32>(sStg, acc0, acc1, c0, r, 1, vh);
-        float a[32];   // group-0 + group-1 columns of channels c0..c0+31
-#pragma unroll
-        for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
-        tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, r, 1, a);
-        if (store) {
-          float o[32];
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
-            if (P.relu) t0 = fmaxf(t0, 0.f);
-            o[c] = t0;
-          }
-          if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + co0 + c0, o, 32);
-          if (P.out_split) {
-            __half* hp = P.out_split + pix * (2 * P.split_c) + co0 + c0;
-            tc::store_split_row<32>(hp, hp + P.split_c, o);
-          }
-        }
-      }
+      E.x0 = tx_ * TW;
+      E.y0 = ty_ * TH;
+      E.b = b;
+      tc::conv_epilogue<NOUT>(acc0, acc1, sStg, piece, srow, E);
     }
+    if (threadIdx.x == 0) tc::bulk_wait_all();
   }
 }
 
@@ -563,6 +554,41 @@ static void pick_tile(int H, int W, int& tw_log2) {
   tw_log2 = best;
 }
 
+int encode_conv_out_maps(PFN_encodeTiled enc, CUtensorMap* smap, __half* out_split, int split_c, CUtensorMap* fmap, float* out_f32,
+                         int f32_c, bool c8, int B, int H, int W, int TW, int TH) {
+  const CUtensorMapSwizzle swz = c8 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_64B;
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  if (out_split) {
+    const cuuint64_t row = (cuuint64_t)2 * split_c * sizeof(__half);
+    XF_REQUIRE(((uintptr_t)out_split & 15) == 0 && row % 16 == 0, "conv_tc: split output %p (row %d B) is not 16-byte aligned",
+               (void*)out_split, (int)row);
+    const cuuint64_t dims[4] = {(cuuint64_t)2 * split_c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {row, (cuuint64_t)W * row, (cuuint64_t)H * W * row};
+    const cuuint32_t box[4] = {c8 ? 16u : 32u, (cuuint32_t)TW, (cuuint32_t)TH, 1};
+    const CUresult r = enc(smap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)out_split, dims, strides, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("cuTensorMapEncodeTiled(split output %dx%dx%dx%d) failed: %d", B, H, W, 2 * split_c, (int)r);
+      return XF_E_CUDA;
+    }
+  }
+  if (out_f32) {
+    const cuuint64_t row = (cuuint64_t)f32_c * sizeof(float);
+    XF_REQUIRE(((uintptr_t)out_f32 & 15) == 0 && row % 16 == 0, "conv_tc: fp32 output %p (row %d B) is not 16-byte aligned",
+               (void*)out_f32, (int)row);
+    const cuuint64_t dims[4] = {(cuuint64_t)f32_c, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {row, (cuuint64_t)W * row, (cuuint64_t)H * W * row};
+    const cuuint32_t box[4] = {c8 ? 8u : 16u, (cuuint32_t)TW, (cuuint32_t)TH, 1};
+    const CUresult r = enc(fmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)out_f32, dims, strides, box, estr,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("cuTensorMapEncodeTiled(fp32 output %dx%dx%dx%d) failed: %d", B, H, W, f32_c, (int)r);
+      return XF_E_CUDA;
+    }
+  }
+  return XF_OK;
+}
+
 template <int KS, int CINP, int NOUT>
 static int launch_tc_cfg(const ConvTcParams& P, int grid, cudaStream_t st) {
   using C = ConvTcCfg<KS, CINP, NOUT>;
@@ -611,9 +637,8 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
   P.stride = S;
   P.pad = sp.ks / 2;
   P.tw_log2 = tw_log2;
-  P.out_split = out_split;
-  P.out_f32 = out_f32;
-  P.f32_c = sp.cout;
+  P.has_split = out_split != nullptr;
+  P.has_f32 = out_f32 != nullptr;
   P.relu = sp.relu;
   P.skip_xn = skip_xn;
   P.skip_w = skip_xn ? ctx->d_weights + ctx->table.w_off[L_SKIP1] : nullptr;   // 24 weights; the 24 biases follow (layers.h packing)
@@ -623,6 +648,8 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
   P.div_x = make_fastdiv((unsigned)cdiv(Wo, TW));
   const int grid = n_tiles < ctx->sm_count ? n_tiles : ctx->sm_count;
   P.split_c = sp.cout <= 32 ? 32 : sp.cout;   // channel count of the split output tensor [hi(split_c) | lo(split_c)]
+  int rc = encode_conv_out_maps(enc, &P.smap, out_split, P.split_c, &P.fmap, out_f32, sp.cout, false, B, Ho, Wo, TW, TH);
+  if (rc) return rc;
   if (c.cinp == 128) {
     const cuuint64_t wdims[2] = {64, (cuuint64_t)c.ntiles * taps * 4 * 64};
     const cuuint64_t wstrides[1] = {128};
@@ -665,7 +692,6 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
     P.bias = ctx->d_weights + ctx->table.b_off[layer] + nt * c.nout;
     P.f32_co0 = nt * c.nout;
     P.n_real = sp.cout - nt * c.nout < c.nout ? sp.cout - nt * c.nout : c.nout;
-    int rc;
     if (sp.ks == 3 && c.cinp == 64 && c.nout == 64) rc = launch_tc_cfg<3, 64, 64>(P, grid, st);
     else if (sp.ks == 1 && c.cinp == 64 && c.nout == 64) rc = launch_tc_cfg<1, 64, 64>(P, grid, st);
     else if (sp.ks == 3 && c.cinp == 32 && c.nout == 32) rc = launch_tc_cfg<3, 32, 32>(P, grid, st);

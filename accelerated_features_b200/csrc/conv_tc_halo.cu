@@ -40,9 +40,10 @@ struct HaloParams {
   float inv_wscale;
   int B, H, W;
   int TW, TH, PW;
-  __half* out_split;
-  float* out_f32;
-  int f32_c, n_real;
+  CUtensorMap smap;   // split output (B,H,W,2*NOUT); box {32, TW, TH, 1} (NOUT = 8: {16, TW, TH, 1})
+  CUtensorMap fmap;   // fp32 output (B,H,W,cout); box {16, TW, TH, 1} (NOUT = 8: {8, TW, TH, 1})
+  int has_split, has_f32;
+  int n_real;
   int relu;
   FastDiv div_img, div_x;
   int desc_mode;      // 0 (default): base_offset = 0; 1: base_offset = (addr >> 7) & 7 (bring-up experiment)
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
   unsigned char* sP = base + C::W_BYTES;                     // patch buffers
   constexpr int NP = C::NP;
   constexpr int PB = C::PB;
-  float* sStg = reinterpret_cast<float*>(base + C::W_BYTES + NP * PB);
+  unsigned char* sStg = base + C::W_BYTES + NP * PB;
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + C::W_BYTES + NP * PB + tc::STG_BYTES);
   uint64_t* w_full = bars;
   uint64_t* p_full = bars + 1;            // [NP]
@@ -85,6 +86,8 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
   if (warp == 4 && lane == 0) {
     tc::tma_prefetch_desc(&P.amap);
     tc::tma_prefetch_desc(&P.wmap);
+    if (P.has_split) tc::tma_prefetch_desc(&P.smap);
+    if (P.has_f32) tc::tma_prefetch_desc(&P.fmap);
     tc::mbar_init(w_full, 1);
     for (int i = 0; i < NP; ++i) {
       tc::mbar_init(&p_full[i], 1);
@@ -127,10 +130,24 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
   } else {
     constexpr int N2 = 2 * NOUT;
     constexpr uint32_t HALF = 64u * ROWB;          // bytes: rows 64-127 of the GEMM
-    const int m = threadIdx.x;                     // GEMM row of this thread = patch-pitch pixel
-    const int mh = m / P.PW, mw = m - mh * P.PW;
-    const bool lane_ok = (mh < P.TH) && (mw < P.TW);
     float acc0[NOUT], acc1[NOUT];
+    int srow[4];   // GEMM row m = h * PW + w -> staging row h * TW + w; rows with w >= TW or h >= TH are junk
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int m = tc::frag_row(threadIdx.x, i), mh = m / P.PW, mw = m - mh * P.PW;
+      srow[i] = (mh < P.TH && mw < P.TW) ? mh * P.TW + mw : -1;
+    }
+    tc::ConvEpi E;
+    E.split = P.has_split ? &P.smap : nullptr;
+    E.f32 = P.has_f32 ? &P.fmap : nullptr;
+    E.split_c = NOUT;
+    E.co = 0;
+    E.inv_wscale = P.inv_wscale;
+    E.relu = P.relu;
+    E.bias = sBias;
+    E.skip_w = nullptr;
+    E.skip_v = nullptr;
+    uint32_t piece = 0;
     const uint32_t w_base = tc::smem_u32(sW);
     tc::mbar_wait(w_full, 0);
     uint32_t tcount = 0;
@@ -214,54 +231,12 @@ __global__ void __launch_bounds__(CH_THREADS, 1) conv_tc_halo_kernel(const __gri
       // ---------------- epilogue ----------------
       const int b = (int)fdiv((unsigned)tile, P.div_img), rem = tile - b * tiles_img;
       const int ty_ = (int)fdiv((unsigned)rem, P.div_x), tx_ = rem - ty_ * tiles_x;
-      const int y = ty_ * P.TH + mh, x = tx_ * P.TW + mw;
-      const bool store = lane_ok && y < P.H && x < P.W;
-      const int64_t pix = ((int64_t)b * P.H + y) * P.W + x;
-      if constexpr (NOUT == 8) {
-        uint32_t v[N2];
-        tc::acc_rows<16>(sStg, acc0, acc1, 0, m, 1, v);
-        if (store) {
-          float o[NOUT];
-#pragma unroll
-          for (int c = 0; c < NOUT; ++c) {
-            float t0 = fmaf(__uint_as_float(v[c]) + __uint_as_float(v[NOUT + c]), P.inv_wscale, sBias[c]);
-            if (P.relu) t0 = fmaxf(t0, 0.f);
-            o[c] = t0;
-          }
-          if (P.out_f32) tc::store_f32_row<NOUT>(P.out_f32 + pix * P.f32_c, o, P.n_real);
-          if (P.out_split) {
-            __half* hp = P.out_split + pix * (2 * NOUT);
-            tc::store_split_row<NOUT>(hp, hp + NOUT, o);
-          }
-        }
-      } else {
-        // 32 output channels at a time: the group-0 columns c and the group-1 columns NOUT + c of the same channels, so that
-        // no copy of all 2 * NOUT accumulator columns sits next to the accumulators
-#pragma unroll
-        for (int c0 = 0; c0 < NOUT; c0 += 32) {
-          uint32_t vh[32];
-          tc::acc_rows<32>(sStg, acc0, acc1, c0, m, 1, vh);
-          float a[32];   // group-0 + group-1 columns of channels c0..c0+31
-#pragma unroll
-          for (int c = 0; c < 32; ++c) a[c] = __uint_as_float(vh[c]);
-          tc::acc_rows_add<32>(sStg, acc0, acc1, NOUT + c0, m, 1, a);
-          if (store) {
-            float o[32];
-#pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              float t0 = fmaf(a[c], P.inv_wscale, sBias[c0 + c]);
-              if (P.relu) t0 = fmaxf(t0, 0.f);
-              o[c] = t0;
-            }
-            if (P.out_f32) tc::store_f32_row<32>(P.out_f32 + pix * P.f32_c + c0, o, P.n_real - c0);
-            if (P.out_split) {
-              __half* hp = P.out_split + pix * (2 * NOUT) + c0;
-              tc::store_split_row<32>(hp, hp + NOUT, o);
-            }
-          }
-        }
-      }
+      E.x0 = tx_ * P.TW;
+      E.y0 = ty_ * P.TH;
+      E.b = b;
+      tc::conv_epilogue<NOUT>(acc0, acc1, sStg, piece, srow, E);
     }
+    if (threadIdx.x == 0) tc::bulk_wait_all();
   }
 }
 
@@ -324,12 +299,13 @@ int launch_conv_tc_halo(const xfeat_ctx* ctx, int layer, const __half* in_split,
   P.bias = ctx->d_weights + ctx->table.b_off[layer];
   P.inv_wscale = ctx->tc_inv_wscale[layer];
   P.B = B; P.H = H; P.W = W;
-  P.out_split = out_split;
-  P.out_f32 = out_f32;
-  P.f32_c = sp.cout;
+  P.has_split = out_split != nullptr;
+  P.has_f32 = out_f32 != nullptr;
   P.n_real = sp.cout;
   P.relu = sp.relu;
   P.desc_mode = g_halo_desc_mode;
+  const int rc = encode_conv_out_maps(enc, &P.smap, out_split, nout, &P.fmap, out_f32, sp.cout, c8, B, H, W, P.TW, P.TH);
+  if (rc) return rc;
   const int n_tiles = cdiv(H, P.TH) * cdiv(W, P.TW) * B;
   XF_REQUIRE(n_tiles < (1 << 22), "conv_tc_halo: too many tiles (%d)", n_tiles);
   P.div_img = make_fastdiv((unsigned)(cdiv(H, P.TH) * cdiv(W, P.TW)));

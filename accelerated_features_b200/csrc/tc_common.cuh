@@ -72,6 +72,19 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// shared -> global box store; the TMA clips the elements that fall outside the tensor
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the stores of all but the newest N committed groups have finished READING shared memory (their source may be rewritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every committed store has completed
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------- wgmma (sm_90a)
 // D[registers] (+)= A[smem] * B[smem] for a 64-row slab, issued collectively by the four warps of one warpgroup.  Thread
@@ -208,20 +221,6 @@ __device__ __forceinline__ void acc_rows(float* stg, const float (&d0)[R], const
   stage_read<CW>(stg, wt, v);
   wg_sync(bar);
 }
-// a[j] += column c0 + j of row `wt`: the split-term epilogues sum the group-0 and group-1 columns of a channel without holding
-// both 32-column chunks in registers at once
-template <int CW, int R>
-__device__ __forceinline__ void acc_rows_add(float* stg, const float (&d0)[R], const float (&d1)[R], int c0, int wt, int bar,
-                                             float (&a)[CW]) {
-  stage_write<CW>(stg, d0, d1, c0, wt);
-  wg_sync(bar);
-#pragma unroll
-  for (int k = 0; k < CW / 4; ++k) {
-    const float4 t = *reinterpret_cast<const float4*>(stg + stg_off(wt, 4 * k));
-    a[4 * k] += t.x; a[4 * k + 1] += t.y; a[4 * k + 2] += t.z; a[4 * k + 3] += t.w;
-  }
-  wg_sync(bar);
-}
 
 // ---------------------------------------------------------------- epilogue stores
 // 32 bytes per thread and call as two 16-byte stores: the conv epilogues write one pixel row per thread, so a warp-wide store
@@ -230,38 +229,24 @@ __device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&v)[8]) {
   reinterpret_cast<uint4*>(p)[0] = make_uint4(v[0], v[1], v[2], v[3]);
   reinterpret_cast<uint4*>(p)[1] = make_uint4(v[4], v[5], v[6], v[7]);
 }
-// N fp32 values -> split fp16 row pieces: hi block at hp, lo block at lp (N halves each), x = hi + lo.  hp / lp 32-byte aligned
-// for N >= 16; N == 8: lp == hp + 8 and the 32-byte row [hi(8) | lo(8)] goes out as one store.
+// N fp32 values -> split fp16 row pieces: hi block at hp, lo block at lp (N halves each, 32-byte aligned), x = hi + lo
 template <int N>
 __device__ __forceinline__ void store_split_row(__half* hp, __half* lp, const float (&o)[N]) {
-  static_assert(N == 8 || N % 16 == 0, "store_split_row: N");
-  if constexpr (N == 8) {
-    uint32_t v[8];
+  static_assert(N % 16 == 0, "store_split_row: N");
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const __half2 h = __floats2half2_rn(o[2 * j], o[2 * j + 1]);
+  for (int c = 0; c < N / 16; ++c) {
+    uint32_t vh[8], vl[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float x0 = o[16 * c + 2 * j], x1 = o[16 * c + 2 * j + 1];
+      const __half2 h = __floats2half2_rn(x0, x1);
       const float2 hf = __half22float2(h);
-      const __half2 l = __floats2half2_rn(o[2 * j] - hf.x, o[2 * j + 1] - hf.y);
-      v[j] = *reinterpret_cast<const uint32_t*>(&h);
-      v[4 + j] = *reinterpret_cast<const uint32_t*>(&l);
+      const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+      vh[j] = *reinterpret_cast<const uint32_t*>(&h);
+      vl[j] = *reinterpret_cast<const uint32_t*>(&l);
     }
-    st_global_v8(hp, v);
-  } else {
-#pragma unroll
-    for (int c = 0; c < N / 16; ++c) {
-      uint32_t vh[8], vl[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float x0 = o[16 * c + 2 * j], x1 = o[16 * c + 2 * j + 1];
-        const __half2 h = __floats2half2_rn(x0, x1);
-        const float2 hf = __half22float2(h);
-        const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-        vh[j] = *reinterpret_cast<const uint32_t*>(&h);
-        vl[j] = *reinterpret_cast<const uint32_t*>(&l);
-      }
-      st_global_v8(hp + 16 * c, vh);
-      st_global_v8(lp + 16 * c, vl);
-    }
+    st_global_v8(hp + 16 * c, vh);
+    st_global_v8(lp + 16 * c, vl);
   }
 }
 // N fp32 values to a 32-byte aligned fp32 row, the first n_real of them (a multiple of 4)
@@ -276,6 +261,133 @@ __device__ __forceinline__ void store_f32_row(float* op, const float (&o)[N], in
       st_global_v8(op + 8 * c, v);
     } else if (8 * c < n_real) {
       reinterpret_cast<float4*>(op + 8 * c)[0] = make_float4(o[8 * c], o[8 * c + 1], o[8 * c + 2], o[8 * c + 3]);
+    }
+  }
+}
+
+// ---------------------------------------------------------------- conv epilogue: fragments -> TMA tensor stores
+// The convolution kernels write a tile's outputs straight from the wgmma fragments: thread (warp w, lane l) holds the group-0
+// column c and the group-1 column NOUT + c of every channel c = 8j + 2(l%4) + e it owns, for rows r, r+8, r+64, r+72
+// (r = 16w + l/4), so the split-term sum needs no transpose.  The values go into a staging PIECE -- 128 pixel rows of RB
+// bytes, pixel-major as the NHWC output, swizzled as the tensor map's SWIZZLE_<RB>B -- that one thread hands to the TMA as a
+// box {channels, TW, TH, 1}.  Pieces alternate between the two halves of the staging region, so piece k+1 is written while the
+// TMA still reads piece k; the TMA clips the box at the image's right and bottom edges.
+constexpr int STG_PIECE = STG_BYTES / 2;
+template <int RB>
+__device__ __forceinline__ uint32_t piece_off(int row, int byte) {   // 16-byte chunk index ^= (byte offset >> 7) % (RB / 16)
+  const uint32_t o = (uint32_t)(row * RB + byte);
+  return o ^ (((o >> 7) & (RB / 16 - 1)) << 4);
+}
+
+struct ConvEpi {
+  const CUtensorMap* split;   // split fp16 output [hi(split_c) | lo(split_c)] or null; boxes of 32 halves (8-ch: 16, a whole row)
+  const CUtensorMap* f32;     // fp32 output or null; boxes of 16 floats (8-ch: 8)
+  int split_c;                // channels per half of a split pixel row
+  int co;                     // output channel of the tile's first accumulator channel
+  float inv_wscale;
+  int relu;
+  const float* bias;          // shared memory [NOUT]
+  const float* skip_w;        // block1.3's skip branch: shared memory [2][NOUT] weights, biases; or null
+  const float* skip_v;        // ... and the pooled input per staging row
+  int x0, y0, b;              // box origin: the tile's first output pixel
+};
+
+// one piece: every thread writes its part, one thread stores it.  `piece` counts the CTA's pieces: before the barrier that
+// publishes piece k, the issuing thread waits until the TMA has read piece k-1, whose half piece k+1 is written into.
+template <class Write>
+__device__ __forceinline__ void conv_store_piece(unsigned char* stg, uint32_t& piece, const CUtensorMap* map, int c, const ConvEpi& E,
+                                                 Write&& write) {
+  unsigned char* buf = stg + (piece & 1) * STG_PIECE;
+  write(buf);
+  fence_proxy_async();   // this thread's generic-proxy writes, before the TMA (async proxy) reads them
+  if (threadIdx.x == 0) bulk_wait_read<0>();
+  wg_sync(1);
+  if (threadIdx.x == 0) {
+    tma_store_4d(map, buf, c, E.x0, E.y0, E.b);
+    bulk_commit();
+  }
+  ++piece;
+}
+
+// Bias, ReLU, block1.3's skip term, then the split x = hi + lo -- per value in the order the model defines.  srow[h] is the
+// staging row of fragment row h (r, r+8, r+64, r+72), or -1 for a GEMM row that is no output pixel (halo junk lanes).
+template <int NOUT>
+__device__ __forceinline__ void conv_epilogue(const float (&d0)[NOUT], const float (&d1)[NOUT], unsigned char* stg, uint32_t& piece,
+                                              const int (&srow)[4], const ConvEpi& E) {
+  static_assert(NOUT == 8 || NOUT == 32 || NOUT == 64, "conv_epilogue: NOUT");
+  constexpr int CB = NOUT < 32 ? NOUT : 32;   // channels per block
+  constexpr int JB = CB / 8;                  // 8-column fragment groups per block
+  constexpr int RB = NOUT < 32 ? 32 : 64;     // staging row bytes
+  constexpr int G1 = NOUT / 8;                // fragment group of the group-1 column of channel 0
+  const int q = threadIdx.x & 3;
+  float sv[4];
+#pragma unroll
+  for (int h = 0; h < 4; ++h) sv[h] = (E.skip_w != nullptr && srow[h] >= 0) ? E.skip_v[srow[h]] : 0.f;
+#pragma unroll
+  for (int cb = 0; cb < NOUT / CB; ++cb) {
+    float o[4][JB][2];
+    uint32_t hi[4][JB], lo[4][JB];
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+#pragma unroll
+      for (int jj = 0; jj < JB; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int j = cb * JB + jj, c = 8 * j + 2 * q + e, i = 2 * (h & 1) + e;
+          const float g0 = (h < 2) ? d0[4 * j + i] : d1[4 * j + i];
+          const float g1 = (h < 2) ? d0[4 * (j + G1) + i] : d1[4 * (j + G1) + i];
+          float t = fmaf(g0 + g1, E.inv_wscale, E.bias[c]);
+          if (E.relu) t = fmaxf(t, 0.f);
+          if (E.skip_w != nullptr) t += fmaf(sv[h], E.skip_w[c], E.skip_w[NOUT + c]);
+          o[h][jj][e] = t;
+        }
+        const __half2 hh = __floats2half2_rn(o[h][jj][0], o[h][jj][1]);
+        const float2 hf = __half22float2(hh);
+        const __half2 ll = __floats2half2_rn(o[h][jj][0] - hf.x, o[h][jj][1] - hf.y);
+        hi[h][jj] = *reinterpret_cast<const uint32_t*>(&hh);
+        lo[h][jj] = *reinterpret_cast<const uint32_t*>(&ll);
+      }
+    }
+    if (E.split != nullptr) {
+      if constexpr (NOUT == 8) {   // one piece of whole [hi(8) | lo(8)] rows
+        conv_store_piece(stg, piece, E.split, 0, E, [&](unsigned char* buf) {
+#pragma unroll
+          for (int h = 0; h < 4; ++h)
+            if (srow[h] >= 0) {
+              *reinterpret_cast<uint32_t*>(buf + piece_off<RB>(srow[h], 4 * q)) = hi[h][0];
+              *reinterpret_cast<uint32_t*>(buf + piece_off<RB>(srow[h], 16 + 4 * q)) = lo[h][0];
+            }
+        });
+      } else {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {   // the hi piece of channels co + 32cb.., then the lo piece
+          conv_store_piece(stg, piece, E.split, half * E.split_c + E.co + CB * cb, E, [&](unsigned char* buf) {
+#pragma unroll
+            for (int h = 0; h < 4; ++h)
+              if (srow[h] >= 0) {
+#pragma unroll
+                for (int jj = 0; jj < JB; ++jj)
+                  *reinterpret_cast<uint32_t*>(buf + piece_off<RB>(srow[h], 16 * jj + 4 * q)) = half ? lo[h][jj] : hi[h][jj];
+              }
+          });
+        }
+      }
+    }
+    if (E.f32 != nullptr) {
+      constexpr int FJ = RB / 32;   // fragment groups per fp32 piece (8 floats = 32 bytes each)
+#pragma unroll
+      for (int k = 0; k < JB / FJ; ++k) {
+        conv_store_piece(stg, piece, E.f32, E.co + CB * cb + 8 * FJ * k, E, [&](unsigned char* buf) {
+#pragma unroll
+          for (int h = 0; h < 4; ++h)
+            if (srow[h] >= 0) {
+#pragma unroll
+              for (int jj = 0; jj < FJ; ++jj)
+                *reinterpret_cast<float2*>(buf + piece_off<RB>(srow[h], 32 * jj + 8 * q)) =
+                    make_float2(o[h][FJ * k + jj][0], o[h][FJ * k + jj][1]);
+            }
+        });
+      }
     }
   }
 }
@@ -327,5 +439,11 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 PFN_encodeTiled get_encode_tiled();
+// Tensor maps of a convolution's NHWC outputs as tc::conv_epilogue stores them: the split fp16 tensor (B,H,W,2*split_c) in
+// boxes {32 halves, TW, TH, 1} and the fp32 tensor (B,H,W,f32_c) in boxes {16 floats, TW, TH, 1}, SWIZZLE_64B; 8-channel
+// layers (c8) use {16 halves} (a whole [hi(8)|lo(8)] row) and {8 floats}, SWIZZLE_32B.  A null output gets no map; an output
+// base or row that is not 16-byte aligned is an error.
+int encode_conv_out_maps(PFN_encodeTiled enc, CUtensorMap* smap, __half* out_split, int split_c, CUtensorMap* fmap, float* out_f32,
+                         int f32_c, bool c8, int B, int H, int W, int TW, int TH);
 
 }  // namespace xf
