@@ -90,6 +90,8 @@ extern "C" int xfeat_detect_dense(xfeat_ctx* ctx, const float* d_feats, const fl
   XF_REQUIRE(out_offset >= 0 && out_offset + k <= out_rows, "detect_dense: output rows [%d,%d) exceed %d", out_offset,
              out_offset + k, out_rows);
   XF_REQUIRE((int64_t)B * cells < (1ll << 31), "detect_dense: batch too large for 32-bit offsets");
+  XF_REQUIRE(((uintptr_t)d_feats | (uintptr_t)d_desc) % 8 == 0,   // the gather moves feature rows as float2
+             "detect_dense: d_feats and d_desc must be 8-byte aligned");
   XF_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   xf::Bump bump(d_ws, ws_bytes);

@@ -777,6 +777,9 @@ extern "C" int xfeat_detect_sparse_split(xfeat_ctx* ctx, const float* d_feats, c
   XF_REQUIRE(B > 0 && B <= 65535 && H > 0 && W > 0 && H % 32 == 0 && W % 32 == 0 && top_k > 0,
              "detect_sparse: bad shape B=%d H=%d W=%d top_k=%d", B, H, W, top_k);
   XF_REQUIRE((int64_t)B * xf::sparse_cap(H, W) < (1ll << 31), "detect_sparse: batch too large for 32-bit offsets");
+  // the NMS reads d_heat and the samplers read d_feats as float4, and store d_desc as float4 and d_desc_split as uint4
+  XF_REQUIRE(((uintptr_t)d_heat | (uintptr_t)d_feats | (uintptr_t)d_desc | (uintptr_t)d_desc_split) % 16 == 0,
+             "detect_sparse: d_heat, d_feats, d_desc and d_desc_split must be 16-byte aligned");
   XF_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   xf::Bump bump(d_ws, ws_bytes);

@@ -115,7 +115,7 @@ XF_API size_t xfeat_sparse_workspace_bytes(int B, int H, int W, int top_k);
  *   of leading entries with score > 0, or XF_N_OVERFLOW when more than H*W/4 candidates with a positive score were found
  *   (all outputs of that image are then zero-filled); d_n_cand (B) int32 = number of NMS maxima above threshold (before the
  *   score filter; for parity checks, may be NULL); d_kpts_int (B,top_k,2) int32 optional. Entries past n_valid
- *   are zero-filled. */
+ *   are zero-filled.  d_heat, d_feats and d_desc must be 16-byte aligned (XF_E_INVALID otherwise). */
 XF_API int xfeat_detect_sparse(xfeat_ctx* ctx, const float* d_feats, const float* d_heat, const float* d_reliability,
                         int B, int H, int W, int top_k, float threshold, float rw, float rh,
                         float* d_kpts, float* d_scores, float* d_desc, int32_t* d_n_valid, int32_t* d_n_cand,
@@ -125,7 +125,8 @@ XF_API int xfeat_detect_sparse(xfeat_ctx* ctx, const float* d_feats, const float
  * descriptor * 2^13 (x = hi + lo; XF_DESC_SPLIT_SCALE_LOG2), rows past n_valid zero; split_rows a multiple of 512, >= top_k.
  * xfeat_mnn_match_presplit consumes them, which removes the max-reduction and split passes of xfeat_mnn_match from the sparse
  * path.  d_desc_split == NULL: identical to xfeat_detect_sparse.  d_desc may be NULL when d_desc_split is given (a caller that only
- * matches does not need the fp32 descriptors: 134 MB of writes less per 128 x 4096 keypoints). */
+ * matches does not need the fp32 descriptors: 134 MB of writes less per 128 x 4096 keypoints).  d_desc_split must be 16-byte
+ * aligned, as d_heat, d_feats and d_desc. */
 #define XF_DESC_SPLIT_SCALE_LOG2 13
 XF_API int xfeat_detect_sparse_split(xfeat_ctx* ctx, const float* d_feats, const float* d_heat, const float* d_reliability,
                               int B, int H, int W, int top_k, float threshold, float rw, float rh, float* d_kpts,
@@ -138,7 +139,7 @@ XF_API size_t xfeat_dense_workspace_bytes(int B, int H, int W, int top_k);
  * Writes k rows per image at row offset `out_offset` of outputs with `out_rows` rows per image:
  *   d_kpts (B,out_rows,2) = (x*8*rw/div_scale, y*8*rh/div_scale); d_desc (B,out_rows,64) un-normalised;
  *   d_scales (B,out_rows) = scale_value (xfeat.py:389-391; may be NULL); order = reliability descending, ties by cell
- *   index ascending. d_topk_idx (B,k) int32 optional. */
+ *   index ascending. d_topk_idx (B,k) int32 optional.  d_feats and d_desc must be 8-byte aligned (XF_E_INVALID otherwise). */
 XF_API int xfeat_detect_dense(xfeat_ctx* ctx, const float* d_feats, const float* d_reliability, int B, int H, int W,
                        int top_k, float rw, float rh, float div_scale, float scale_value, int out_rows, int out_offset,
                        float* d_kpts, float* d_desc, float* d_scales, int32_t* d_topk_idx, void* d_ws, size_t ws_bytes,
