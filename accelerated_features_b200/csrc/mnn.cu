@@ -227,11 +227,11 @@ static void carve_mnn(Bump& bump, int batch, int n1_max, int n2_max, MnnWs& ws) 
 size_t mnn_tc_workspace_bytes(int batch, int n1_max, int n2_max);
 int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                   int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                  unsigned long long** best21, float** inv_s2, cudaStream_t st, int once, float abs_bound);
-// 0 = fp32 CUDA cores, 1 = wgmma split-fp16 with one GEMM per direction (default), 2 = wgmma single pass: one GEMM, the
-// column arg-max by cross-lane reduction in the epilogue -- same results, but the epilogue then out-weighs the saved GEMM
-// (64 x 4096 x 4096: 0.75 ms vs 0.68 ms per call, tools/mnn_ab.py), so it is kept selectable, not default;
-// 3 = implementation 1 with one CTA per (row block, pair, direction) instead of the persistent kernel
+                  unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant, float abs_bound);
+// 0 = fp32 CUDA cores; 1 = wgmma split-fp16, persistent, ONE GEMM per pair whose accumulator tiles give both the row and the
+// column arg-max, the two consumer warpgroups' epilogues overlapped with each other's MMAs (default); 2 = the persistent
+// kernel with one GEMM per direction -- same results, kept as the reference implementation 1 is compared against;
+// 3 = one CTA per (row block, pair, direction), one GEMM per direction
 // 4 = filter + exact re-score (mnn_fast.cu): one fp16 pass per direction tracking top-1 / top-2, the three-term kernel only on
 // the rows whose gap is within the rounding bound -- same results as 1.  Measured (profiles/r02/mnn_probe.json, 64 x 4096^2):
 // the filter pass is bound by the ALU pipe (FMNMX at 16 lanes/clk: 370 us against 115 us of tensor time), and the descriptors of
@@ -242,7 +242,7 @@ static int g_mnn_impl = 1;
 size_t mnn_fast_workspace_bytes(int batch, int n1_max, int n2_max);
 int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const __half* f2s, const int* n2, int n2_max, int n_pad,
                            int batch, int scale_log2, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int pairs_kernel);
+                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant);
 int launch_mnn_fast(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                     int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
                     unsigned long long** best21, float** inv_s2, cudaStream_t st, float abs_bound, int sm_count);
@@ -297,7 +297,7 @@ extern "C" int xfeat_mnn_match_bounded(const float* d_f1, const int32_t* d_n1, i
     unsigned long long *b12 = nullptr, *b21 = nullptr;
     float* inv_s2 = nullptr;
     int rc = xf::launch_mnn_tc(d_f1, d_n1, n1_max, stride1, d_f2, d_n2, n2_max, stride2, batch, d_ws, ws_bytes, &b12, &b21,
-                               &inv_s2, st, xf::g_mnn_impl == 2 ? 1 : (xf::g_mnn_impl == 3 ? 2 : 0), abs_bound);
+                               &inv_s2, st, xf::g_mnn_impl - 1, abs_bound);
     if (rc) return rc;
     xf::mnn_finalize_kernel<<<batch, 1024, 0, st>>>(b12, b21, d_n1, d_n2, n1_max, n2_max, min_cossim, inv_s2, (long long*)d_idx0,
                                                     (long long*)d_idx1, d_n_matches);
@@ -338,15 +338,15 @@ extern "C" int xfeat_mnn_match_presplit(const void* d_f1s, const int32_t* d_n1, 
   XF_REQUIRE(d_f1s && d_f2s && d_idx0 && d_idx1 && d_n_matches && d_ws, "mnn_match_presplit: null pointer");
   XF_REQUIRE(batch > 0 && batch <= 65535 && n1_max > 0 && n2_max > 0, "mnn_match_presplit: bad sizes");
   XF_REQUIRE(((uintptr_t)d_f1s % 128) == 0 && ((uintptr_t)d_f2s % 128) == 0, "mnn_match_presplit: operands must be 128-byte aligned");
-  if (xf::g_mnn_impl != 1 && xf::g_mnn_impl != 3) {
-    xf::set_error("mnn_match_presplit: implementation %d does not take pre-split operands (1 and 3 do)", xf::g_mnn_impl);
+  if (xf::g_mnn_impl < 1 || xf::g_mnn_impl > 3) {
+    xf::set_error("mnn_match_presplit: implementation %d does not take pre-split operands (1, 2 and 3 do)", xf::g_mnn_impl);
     return XF_E_UNSUPPORTED;
   }
   cudaStream_t st = (cudaStream_t)stream;
   unsigned long long *b12 = nullptr, *b21 = nullptr;
   float* inv_s2 = nullptr;
   int rc = xf::launch_mnn_tc_presplit((const __half*)d_f1s, d_n1, n1_max, (const __half*)d_f2s, d_n2, n2_max, n_pad, batch,
-                                      scale_log2, d_ws, ws_bytes, &b12, &b21, &inv_s2, st, xf::g_mnn_impl == 3);
+                                      scale_log2, d_ws, ws_bytes, &b12, &b21, &inv_s2, st, xf::g_mnn_impl - 1);
   if (rc) return rc;
   xf::mnn_finalize_kernel<<<batch, 1024, 0, st>>>(b12, b21, d_n1, d_n2, n1_max, n2_max, min_cossim, inv_s2, (long long*)d_idx0,
                                                   (long long*)d_idx1, d_n_matches);

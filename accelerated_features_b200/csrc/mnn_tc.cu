@@ -95,7 +95,7 @@ constexpr uint32_t MT_HALF = (64 * 128) >> 4;   // descriptor offset of rows 64-
 
 // three-term S tile of one slab: hi.hi + (dir ? lo.hi, hi.lo : hi.lo, lo.hi), both directions in the same order so that
 // S12[i][j] and S21[j][i] come out of the same three products
-__device__ __forceinline__ void mnn_tile_mma(float (&acc0)[64], float (&acc1)[64], uint32_t a_slab, uint32_t b_stage, int dir) {
+__device__ __forceinline__ void mnn_tile_mma_issue(float (&acc0)[64], float (&acc1)[64], uint32_t a_slab, uint32_t b_stage, int dir) {
   const int a_sel[3] = {0, dir ? 1 : 0, dir ? 0 : 1};
   const int b_sel[3] = {0, dir ? 0 : 1, dir ? 1 : 0};
   tc::wgmma_fence();
@@ -110,6 +110,9 @@ __device__ __forceinline__ void mnn_tile_mma(float (&acc0)[64], float (&acc1)[64
     }
   }
   tc::wgmma_commit();
+}
+__device__ __forceinline__ void mnn_tile_mma(float (&acc0)[64], float (&acc1)[64], uint32_t a_slab, uint32_t b_stage, int dir) {
+  mnn_tile_mma_issue(acc0, acc1, a_slab, b_stage, dir);
   tc::wgmma_wait<0>();
   tc::acc_fence(acc0);
   tc::acc_fence(acc1);
@@ -232,14 +235,15 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_kernel(const __grid_cons
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Persistent form of mnn_tc_kernel: one CTA per SM walks work items (pair, direction, 256-row block) instead of one CTA per
-// item, so barrier initialisation and -- above all -- the 64 KB A-slab load of the NEXT item overlap the tiles of the current
-// one (A slabs double buffered, 3-stage ring of B tiles).  Same arithmetic, same results.
+// Persistent form of mnn_tc_kernel (implementation 2, the reference of the single-GEMM kernel below): one CTA per SM walks
+// work items (pair, direction, 256-row block) instead of one CTA per item, so barrier initialisation and -- above all -- the
+// 64 KB A-slab load of the NEXT item overlap the tiles of the current one (A slabs double buffered, 3-stage ring of B tiles).
+// Same arithmetic, same results.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int TCP_NSB = 3;
 constexpr size_t TCP_SMEM = 1024 + (size_t)(8 + 2 * TCP_NSB) * TC_BOX_BYTES + 256;
 
-__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
+__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __grid_constant__ TcMaps maps,
                                                                        const int* __restrict__ n1p, int n1_max,
                                                                        const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
                                                                        unsigned long long* __restrict__ best12,
@@ -352,44 +356,128 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Single-pass variant (xfeat_set_mnn_impl(2)): S is computed ONCE; the same accumulator tile yields the running row arg-max
-// (as above) and the column arg-max: per column, the thread's best of its four rows (rows ascending: first index wins), a
-// packed (value, ~row) maximum across the eight row lanes of the warp (shuffles), across the CTA's eight warps in shared memory
-// (64-bit atomicMax), then one global 64-bit atomicMax per column and tile -- the packed format mnn_tc_kernel's second
-// direction produces, so mnn_finalize_kernel is unchanged and the result is identical.
+// Default kernel (implementation 1): S = F1.F2^T is computed ONCE per pair, in the three-term order of mnn_tile_mma(dir = 0),
+// and the same accumulator tile yields both arg-maxes.  Persistent CTAs walk items (pair, 256-row block of set 1); an item
+// streams every 128-column B tile of set 2.
+//
+// Ping-pong: the two consumer warpgroups (one 128-row slab each) take turns issuing their MMAs on a B tile (named barriers 1
+// and 2 pass the turn), so warpgroup 0 reduces tile t while the tensor pipe runs warpgroup 1's MMAs on t, and warpgroup 1
+// reduces t while warpgroup 0's MMAs on t+1 run.  A B stage is released once all eight consumer warps' MMAs on it retired.
+//
+// Epilogue of one slab tile, per thread 4 rows x 32 columns:
+//   rows:    value-only running maximum (fmaxf over the thread's columns, then the quad of lanes that shares the row); the
+//            column index is looked up -- first equal column, ascending -- only for rows whose tile maximum beats the running
+//            best (strictly: an earlier tile keeps a tie).
+//   columns: first maximum over the thread's rows r, r+8, r+64, r+72 (ascending, strict >), fp32 maximum across the 8 row
+//            lanes, then the lowest row that holds it (integer minimum over the lanes that match); the four warps' (value,
+//            row) partials meet in shared memory behind a 128-thread barrier, and one red.global.max.u64 per column and slab
+//            merges them into best21 as packed (value, ~row) -- the format and tie rule of a row arg-max of S21, which
+//            mnn_finalize_kernel reads.  The packed max is associative and commutative: the atomic order does not matter.
+// Columns past n2 (last tile) and rows past n1 (last row block) are set to -inf before the reductions.
+//
+// Shared memory: A double buffered across items (2 x 64 KB), a 2-stage B ring (2 x 32 KB), the column partials
+// [slab][tile parity][warp][column] (float value, int row) = 16 KB.  A third B stage does not fit beside the partials
+// (227 KB per block); with both directions in one item the ring only has to cover the load of tile t+2 during the two
+// slabs' MMAs on tile t+1.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr size_t TC1_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256 + 2 * 128 * 8;
+constexpr int TCF_NSB = 2;
+constexpr size_t TCF_COL_BYTES = 2 * 2 * 4 * 128 * sizeof(float2);
+constexpr size_t TCF_SMEM = 1024 + (size_t)(8 + 2 * TCF_NSB) * TC_BOX_BYTES + 256 + TCF_COL_BYTES;
 
-__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_once_kernel(const __grid_constant__ TcMaps maps,
-                                                                    const int* __restrict__ n1p, int n1_max,
-                                                                    const int* __restrict__ n2p, int n2_max, int n_pad,
-                                                                    unsigned long long* __restrict__ best12,
-                                                                    unsigned long long* __restrict__ best21) {
-  const int pair = blockIdx.y;
-  const int n_rows = n1p ? min(n1p[pair], n1_max) : n1_max;
-  const int n_cols = n2p ? min(n2p[pair], n2_max) : n2_max;
-  const int row0 = blockIdx.x * TC_ROWS;
-  if (row0 >= n_rows) return;
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
+// fragment element (h, j, e) as an lvalue (see tc::frag_val)
+__device__ __forceinline__ float& frag_ref(float (&d0)[64], float (&d1)[64], int h, int j, int e) {
+  return (h < 2) ? d0[4 * j + 2 * h + e] : d1[4 * j + 2 * (h - 2) + e];
+}
+
+// running row maximum of the thread's four rows: bv = value, bc = column (first index on ties)
+__device__ __forceinline__ void mnn_row_update(const float (&acc0)[64], const float (&acc1)[64], int col0, int lane,
+                                               float (&bv)[4], int (&bc)[4]) {
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    float m[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      m[q] = fmaxf(fmaxf(tc::frag_val(acc0, acc1, h, 2 * q, 0), tc::frag_val(acc0, acc1, h, 2 * q, 1)),
+                   fmaxf(tc::frag_val(acc0, acc1, h, 2 * q + 1, 0), tc::frag_val(acc0, acc1, h, 2 * q + 1, 1)));
+    float mx = fmaxf(fmaxf(fmaxf(m[0], m[1]), fmaxf(m[2], m[3])), fmaxf(fmaxf(m[4], m[5]), fmaxf(m[6], m[7])));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const bool upd = mx > bv[h];
+    if (__any_sync(0xffffffffu, upd)) {
+      int c = 1 << 30;
+#pragma unroll
+      for (int j = 15; j >= 0; --j)
+#pragma unroll
+        for (int e = 1; e >= 0; --e) c = (tc::frag_val(acc0, acc1, h, j, e) == mx) ? 8 * j + e : c;
+      c += cq;
+      c = min(c, __shfl_xor_sync(0xffffffffu, c, 1));
+      c = min(c, __shfl_xor_sync(0xffffffffu, c, 2));
+      if (upd) {
+        bv[h] = mx;
+        bc[h] = col0 + c;
+      }
+    }
+  }
+}
+
+// column maxima of one tile over the warp's 32 rows of the slab: sc[column] = (value, row within the slab of its first row)
+__device__ __forceinline__ void mnn_col_warp(const float (&acc0)[64], const float (&acc1)[64], int wt, float2* sc) {
+  const int lane = wt & 31, cq = 2 * (lane & 3);
+  const int r0 = 16 * (wt >> 5) + (lane >> 2);   // row of h = 0; h = 1..3 are r0 + 8, r0 + 64, r0 + 72
+#pragma unroll
+  for (int j = 0; j < 16; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      float m = tc::frag_val(acc0, acc1, 0, j, e);
+      int k = 0;
+      const float v1 = tc::frag_val(acc0, acc1, 1, j, e), v2 = tc::frag_val(acc0, acc1, 2, j, e),
+                  v3 = tc::frag_val(acc0, acc1, 3, j, e);
+      if (v1 > m) { m = v1; k = 8; }
+      if (v2 > m) { m = v2; k = 64; }
+      if (v3 > m) { m = v3; k = 72; }
+      float mx = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 8));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 16));
+      int r = (m == mx) ? r0 + k : 1 << 30;
+      r = min(r, __shfl_xor_sync(0xffffffffu, r, 4));
+      r = min(r, __shfl_xor_sync(0xffffffffu, r, 8));
+      r = min(r, __shfl_xor_sync(0xffffffffu, r, 16));
+      if (lane < 4) sc[8 * j + cq + e] = make_float2(mx, __int_as_float(r));
+    }
+}
+
+__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
+                                                                       const int* __restrict__ n1p, int n1_max,
+                                                                       const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
+                                                                       unsigned long long* __restrict__ best12,
+                                                                       unsigned long long* __restrict__ best21) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* sA = base;                       // [slab 2][hi, lo] boxes
-  unsigned char* sB = base + 4 * TC_BOX_BYTES;    // [stage 2][hi, lo] boxes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + 8 * TC_BOX_BYTES);
-  uint64_t* a_full = bars;
-  uint64_t* b_full = bars + 1;     // [2]
-  uint64_t* b_empty = bars + 3;    // [2]
-  unsigned long long* sCol = reinterpret_cast<unsigned long long*>(base + 8 * TC_BOX_BYTES + 256);   // [tile parity 2][128 columns]
+  unsigned char* sA = base;                       // [buffer 2][slab 2][hi, lo] boxes
+  unsigned char* sB = base + 8 * TC_BOX_BYTES;    // [stage TCF_NSB][hi, lo] boxes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (8 + 2 * TCF_NSB) * TC_BOX_BYTES);
+  uint64_t* a_full = bars;                        // [2]
+  uint64_t* a_empty = bars + 2;                   // [2]
+  uint64_t* b_full = bars + 4;                    // [TCF_NSB]
+  uint64_t* b_empty = b_full + TCF_NSB;           // [TCF_NSB]
+  float2* sCol = reinterpret_cast<float2*>(base + (8 + 2 * TCF_NSB) * TC_BOX_BYTES + 256);   // [slab 2][parity 2][warp 4][128]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = (n_cols + TC_BN - 1) / TC_BN;
+  const int RB = n_pad / TC_ROWS;
+  const int n_items = batch * RB;
 
-  for (int i = threadIdx.x; i < 256; i += MT_THREADS) sCol[i] = 0ull;
   if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(&maps.m1);
     tc::tma_prefetch_desc(&maps.m2);
-    tc::mbar_init(a_full, 1);
     for (int i = 0; i < 2; ++i) {
+      tc::mbar_init(&a_full[i], 1);
+      tc::mbar_init(&a_empty[i], 8);
+    }
+    for (int i = 0; i < TCF_NSB; ++i) {
       tc::mbar_init(&b_full[i], 1);
       tc::mbar_init(&b_empty[i], 8);
     }
@@ -397,84 +485,129 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_once_kernel(const __grid
   }
   __syncthreads();
 
+  // item -> (pair, row block); every role walks the same sequence and skips the same (empty) items
+  auto decode = [&](int item, int& pair, int& row0, int& n_rows, int& n_cols) {
+    pair = item / RB;
+    row0 = (item - pair * RB) * TC_ROWS;
+    n_rows = n1p ? min(__ldg(n1p + pair), n1_max) : n1_max;
+    n_cols = n2p ? min(__ldg(n2p + pair), n2_max) : n2_max;
+    return row0 < n_rows && n_cols > 0;
+  };
+
   if (warp == 8) {
-    if (T > 0 && tc::elect_one()) {
-      const int arow = pair * n_pad + row0;
-      tc::mbar_expect_tx(a_full, 4 * TC_BOX_BYTES);
-      for (int slab = 0; slab < 2; ++slab)
-        for (int kb = 0; kb < 2; ++kb)
-          tc::tma_load_2d(sA + (slab * 2 + kb) * TC_BOX_BYTES, &maps.m1, a_full, kb * 64, arow + slab * 128);
-      const int brow = pair * n_pad;
-      for (int t = 0; t < T; ++t) {
-        const int s = t & 1;
-        tc::mbar_wait(&b_empty[s], ((t >> 1) & 1) ^ 1);
-        tc::mbar_expect_tx(&b_full[s], 2 * TC_BOX_BYTES);
-        for (int kb = 0; kb < 2; ++kb)
-          tc::tma_load_2d(sB + (s * 2 + kb) * TC_BOX_BYTES, &maps.m2, &b_full[s], kb * 64, brow + t * TC_BN);
+    if (tc::elect_one()) {
+      uint32_t ai = 0, bi = 0;
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        int pair, row0, n_rows, n_cols;
+        if (!decode(item, pair, row0, n_rows, n_cols)) continue;
+        const int T = (n_cols + TC_BN - 1) / TC_BN;
+        const int ab = ai & 1;
+        tc::mbar_wait(&a_empty[ab], ((ai >> 1) & 1) ^ 1);
+        tc::mbar_expect_tx(&a_full[ab], 4 * TC_BOX_BYTES);
+        const int arow = pair * n_pad + row0;
+        for (int slab = 0; slab < 2; ++slab)
+          for (int kb = 0; kb < 2; ++kb)
+            tc::tma_load_2d(sA + ((ab * 2 + slab) * 2 + kb) * TC_BOX_BYTES, &maps.m1, &a_full[ab], kb * 64, arow + slab * 128);
+        ++ai;
+        const int brow = pair * n_pad;
+        for (int t = 0; t < T; ++t, ++bi) {
+          const int s = bi % TCF_NSB;
+          tc::mbar_wait(&b_empty[s], ((bi / TCF_NSB) & 1) ^ 1);
+          tc::mbar_expect_tx(&b_full[s], 2 * TC_BOX_BYTES);
+          for (int kb = 0; kb < 2; ++kb)
+            tc::tma_load_2d(sB + (s * 2 + kb) * TC_BOX_BYTES, &maps.m2, &b_full[s], kb * 64, brow + t * TC_BN);
+        }
       }
     }
     __syncwarp();
   } else {
-    const int slab = warp >> 2, wt = threadIdx.x & 127, et = threadIdx.x;
-    const int cq = 2 * (lane & 3);
+    const int slab = warp >> 2, wt = threadIdx.x & 127, cq = 2 * (lane & 3);
+    const int my_turn = 1 + slab, next_turn = 2 - slab;   // named barriers: warpgroup 0 issues on 1, warpgroup 1 on 2
     float acc0[64], acc1[64];
-    unsigned long long best[4] = {0ull, 0ull, 0ull, 0ull};
-    bool rvalid[4];
+    uint32_t ai = 0, bi = 0;
+    if (slab == 1) named_arrive(1, 256);   // warpgroup 0 goes first
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+      int pair, row0, n_rows, n_cols;
+      if (!decode(item, pair, row0, n_rows, n_cols)) continue;
+      const int T = (n_cols + TC_BN - 1) / TC_BN;
+      const int ab = ai & 1;
+      const int srow0 = row0 + slab * 128;
+      bool rvalid[4];
 #pragma unroll
-    for (int h = 0; h < 4; ++h) rvalid[h] = row0 + slab * 128 + tc::frag_row(wt, h) < n_rows;
-    if (T > 0) tc::mbar_wait(a_full, 0);
-    const uint32_t a_slab = tc::smem_u32(sA + slab * 2 * TC_BOX_BYTES);
-    for (int t = 0; t < T; ++t) {
-      const int s = t & 1;
-      tc::mbar_wait(&b_full[s], (t >> 1) & 1);
-      mnn_tile_mma(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), 0);
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&b_empty[s]);
-      mnn_row_argmax(acc0, acc1, t * TC_BN, n_cols - t * TC_BN, lane, best);
-      // column arg-max of the tile
-      unsigned long long* sc = sCol + s * 128;
-#pragma unroll
-      for (int j = 0; j < 16; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float m = -INFINITY;
-          int hb = -1;
-#pragma unroll
-          for (int h = 0; h < 4; ++h) {
-            const float v = tc::frag_val(acc0, acc1, h, j, e);
-            if (rvalid[h] && v > m) { m = v; hb = h; }   // rows ascending in h: first index wins ties
-          }
-          unsigned long long p = (hb >= 0) ? pack_vi(m, (uint32_t)(row0 + slab * 128 + tc::frag_row(wt, hb))) : 0ull;
-#pragma unroll
-          for (int o = 4; o <= 16; o <<= 1) {
-            const unsigned long long q = __shfl_xor_sync(0xffffffffu, p, o);
-            p = q > p ? q : p;
-          }
-          if (lane < 4 && p) atomicMax(sc + 8 * j + cq + e, p);
+      for (int h = 0; h < 4; ++h) rvalid[h] = srow0 + tc::frag_row(wt, h) < n_rows;
+      const bool rows_partial = srow0 + 128 > n_rows;
+      tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
+      const uint32_t a_slab = tc::smem_u32(sA + (ab * 2 + slab) * 2 * TC_BOX_BYTES);
+      float bv[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+      int bc[4] = {0, 0, 0, 0};
+      for (int t = 0; t < T; ++t, ++bi) {
+        const int s = bi % TCF_NSB;
+        tc::mbar_wait(&b_full[s], (bi / TCF_NSB) & 1);
+        named_sync(my_turn, 256);
+        mnn_tile_mma_issue(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), 0);
+        named_arrive(next_turn, 256);
+        tc::wgmma_wait<0>();
+        tc::acc_fence(acc0);
+        tc::acc_fence(acc1);
+        __syncwarp();
+        if (lane == 0) {
+          tc::mbar_arrive(&b_empty[s]);
+          if (t == T - 1) tc::mbar_arrive(&a_empty[ab]);   // the A slabs may be overwritten
         }
-      asm volatile("bar.sync 2, 256;" ::: "memory");   // the tile's column maxima of all eight warps are in sCol[s]
-      if (et < 128) {
-        const unsigned long long p = sc[et];
-        if (p && t * TC_BN + et < n_cols) atomicMax(best21 + (int64_t)pair * n2_max + t * TC_BN + et, p);
-        sc[et] = 0ull;   // parity s is written again for tile t+2, after the barrier of tile t+1, which this thread joins later
-      }
-    }
-    if ((lane & 3) == 0) {
+        const int col0 = t * TC_BN, n_valid = n_cols - col0;
+        if (n_valid < TC_BN) {
 #pragma unroll
-      for (int h = 0; h < 4; ++h) {
-        const int row = row0 + slab * 128 + tc::frag_row(wt, h);
-        if (row < n_rows) best12[(int64_t)pair * n1_max + row] = best[h];
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              if (8 * j + cq + e >= n_valid)
+#pragma unroll
+                for (int h = 0; h < 4; ++h) frag_ref(acc0, acc1, h, j, e) = -INFINITY;
+        }
+        if (rows_partial) {
+#pragma unroll
+          for (int h = 0; h < 4; ++h)
+            if (!rvalid[h])
+#pragma unroll
+              for (int j = 0; j < 16; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) frag_ref(acc0, acc1, h, j, e) = -INFINITY;
+        }
+        mnn_row_update(acc0, acc1, col0, lane, bv, bc);
+        float2* sc = sCol + (slab * 2 + (bi & 1)) * 4 * 128;
+        mnn_col_warp(acc0, acc1, wt, sc + (wt >> 5) * 128);
+        tc::wg_sync(3 + slab);   // the four warps' partials of this tile are in sc; parity bi & 1 is written again two tiles on
+        if (wt < n_valid) {
+          unsigned long long p = 0ull;
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {
+            const float2 q = sc[w * 128 + wt];
+            if (q.x != -INFINITY) {
+              const unsigned long long c = pack_vi(q.x, (uint32_t)(srow0 + __float_as_int(q.y)));
+              p = c > p ? c : p;
+            }
+          }
+          if (p) atomicMax(best21 + (int64_t)pair * n2_max + col0 + wt, p);
+        }
+      }
+      ++ai;
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h)
+          if (rvalid[h]) best12[(int64_t)pair * n1_max + srow0 + tc::frag_row(wt, h)] = pack_vi(bv[h], (uint32_t)bc[h]);
       }
     }
+    if (slab == 0) named_sync(1, 256);   // warpgroup 1's last hand-over
   }
 }
 
-// Both directions of the three-term scan over the full sets: the persistent kernel (default), or one CTA per (row block, pair,
-// direction) with `oneshot` (implementation 3) or XFEAT_MNN_ONESHOT=1.
+// The three-term scan of both directions over the full sets.  variant 0 (implementation 1, default): the single-GEMM persistent
+// kernel; 1 (implementation 2): the persistent kernel with one GEMM per direction; 2 (implementation 3) or XFEAT_MNN_ONESHOT=1:
+// one CTA per (row block, pair, direction).
 static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, const int* n2, int n2_max, int n_pad, int batch,
-                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st, bool oneshot = false) {
+                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st, int variant) {
   static const bool oneshot_env = getenv("XFEAT_MNN_ONESHOT") != nullptr;
-  if (oneshot || oneshot_env) {
+  if (variant == 2 || oneshot_env) {
     XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
     dim3 grid(n_pad / TC_ROWS, batch, 2);
     TcMaps4 m4;
@@ -486,10 +619,17 @@ static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, con
   int dev = 0, sms = 148;
   XF_CUDA(cudaGetDevice(&dev));
   XF_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  XF_DYN_SMEM(mnn_tc_persist_kernel, TCP_SMEM);
-  const int n_items = batch * 2 * (n_pad / TC_ROWS);
-  mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCP_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch, best12,
-                                                                                    best21);
+  if (variant == 1) {
+    XF_DYN_SMEM(mnn_tc_persist2_kernel, TCP_SMEM);
+    const int n_items = batch * 2 * (n_pad / TC_ROWS);
+    mnn_tc_persist2_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCP_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
+                                                                                       best12, best21);
+  } else {
+    XF_DYN_SMEM(mnn_tc_persist_kernel, TCF_SMEM);
+    const int n_items = batch * (n_pad / TC_ROWS);
+    mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCF_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
+                                                                                      best12, best21);
+  }
   XF_LAUNCH_CHECK();
   return XF_OK;
 }
@@ -541,7 +681,7 @@ static int make_map(CUtensorMap* m, const __half* ptr, uint64_t rows) {
 // Fills best12 (rows of F1 -> arg-max column in F2) and best21 (rows of F2 -> arg-max in F1), packed (value*s^2, index).
 int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                   int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                  unsigned long long** best21, float** inv_s2, cudaStream_t st, int once, float abs_bound) {
+                  unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant, float abs_bound) {
   Bump bump(d_ws, ws_bytes);
   MnnTcWs ws;
   carve_mnn_tc(bump, batch, n1_max, n2_max, ws);
@@ -567,21 +707,12 @@ int launch_mnn_tc(const float* f1, const int* n1, int n1_max, int64_t stride1, c
   int rc;
   if ((rc = make_map(&maps.m1, ws.f1s, (uint64_t)batch * n_pad))) return rc;
   if ((rc = make_map(&maps.m2, ws.f2s, (uint64_t)batch * n_pad))) return rc;
-  XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
-  XF_DYN_SMEM(mnn_tc_once_kernel, TC1_SMEM);
   XF_CUDA(cudaMemsetAsync(ws.best12, 0, sizeof(unsigned long long) * (size_t)batch * n1_max, st));
   *inv_s2 = ws.inv_s2;
   *best12 = ws.best12;
   *best21 = ws.best21;
   XF_CUDA(cudaMemsetAsync(ws.best21, 0, sizeof(unsigned long long) * (size_t)batch * n2_max, st));
-  if (once == 2) return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, ws.best12, ws.best21, st, true);
-  if (once) {
-    dim3 grid1(n_pad / TC_ROWS, batch);
-    mnn_tc_once_kernel<<<grid1, MT_THREADS, TC1_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, ws.best12, ws.best21);
-    XF_LAUNCH_CHECK();
-    return XF_OK;
-  }
-  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, ws.best12, ws.best21, st);
+  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, ws.best12, ws.best21, st, variant);
 }
 
 int launch_mnn_tc_rows(const __half* a0, const __half* b0, const __half* a1, const __half* b1, const int* n1, int n1_max,
@@ -592,7 +723,7 @@ __global__ void set_scalar_kernel(float* p, float v) { *p = v; }
 // Operands already split by the producer (xfeat_detect_sparse_split): (batch * n_pad) rows x 128 halves each, scaled by 2^scale_log2.
 int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const __half* f2s, const int* n2, int n2_max, int n_pad,
                            int batch, int scale_log2, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int pairs_kernel) {
+                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant) {
   XF_REQUIRE(n_pad % (2 * TC_ROWS) == 0 && n_pad >= n1_max && n_pad >= n2_max, "mnn_match_presplit: n_pad must be a multiple of %d covering both sets", 2 * TC_ROWS);
   XF_REQUIRE((int64_t)batch * n_pad < (1ll << 31), "mnn_match_presplit: batch * n too large");
   Bump bump(d_ws, ws_bytes);
@@ -612,7 +743,7 @@ int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const _
   int rc;
   if ((rc = make_map(&maps.m1, f1s, (uint64_t)batch * n_pad))) return rc;
   if ((rc = make_map(&maps.m2, f2s, (uint64_t)batch * n_pad))) return rc;
-  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, pairs_kernel != 0);
+  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, variant);
 }
 
 int launch_absmax(const float* f, const int* np, int n_max, int64_t stride, int batch, unsigned* out, cudaStream_t st) {

@@ -384,7 +384,7 @@ class XFeat(torch.nn.Module):
         if x2.shape[0] != B:
             raise RuntimeError("the two image sets must have the same batch size")
         if x1.shape[1:] == x2.shape[1:]:
-            presplit = self._lib.xfeat_get_mnn_impl() in (1, 3)     # the sampler writes the matcher's operand rows itself
+            presplit = self._lib.xfeat_get_mnn_impl() in (1, 2, 3)     # the sampler writes the matcher's operand rows itself
             o = self._detect_sparse_device([x1, x2], top_k, self.detection_threshold, [da, db], want_split=presplit,
                                            want_desc=not presplit)
             k1, k2 = o["keypoints"][:B], o["keypoints"][B:]

@@ -92,7 +92,7 @@ def main():
     g = torch.Generator().manual_seed(1000)
     d1 = torch.randn(BATCH, 3, H, W, generator=g).to(dev)
     d2 = torch.randn(BATCH, 3, H, W, generator=g).to(dev)
-    presplit = lib.xfeat_get_mnn_impl() in (1, 3)
+    presplit = lib.xfeat_get_mnn_impl() in (1, 2, 3)
 
     def step():
         o = xf._detect_sparse_device([d1, d2], TOPK, xf.detection_threshold, want_split=presplit, want_desc=not presplit)

@@ -1,6 +1,8 @@
 #!/usr/bin/env python
-"""A/B timing of the three xfeat_mnn_match implementations on the BASELINE config-2 matching load (64 pairs x 4096 x 4096).
-    python tools/mnn_ab.py            -> one JSON line: ms per call for impl 0 (fp32 SIMT), 1 (tcgen05, two GEMMs), 2 (single pass), 3 (CTA pairs)"""
+"""A/B timing of the xfeat_mnn_match implementations on the BASELINE config-2 matching load (64 pairs x 4096 x 4096), in one
+process.  python tools/mnn_ab.py  -> one JSON line: ms per call for impl 1 (wgmma, one GEMM per pair, default), 2 (wgmma,
+persistent, one GEMM per direction), 3 (one CTA per row block and direction) and 0 (fp32 SIMT), and whether each returns
+what impl 1 returns."""
 import json
 import os
 import sys
@@ -18,7 +20,7 @@ f1 = F.normalize(torch.randn(B, N, 64, generator=g), dim=-1).cuda()
 f2 = F.normalize(torch.randn(B, N, 64, generator=g), dim=-1).cuda()
 out = {}
 ref = None
-for impl in (1, 3, 2, 0):
+for impl in (1, 2, 3, 0):
     xf._lib.xfeat_set_mnn_impl(impl)
     for _ in range(3):
         r = xf._mnn_device(f1, None, N, N * 64, f2, None, N, N * 64, B, -1)
