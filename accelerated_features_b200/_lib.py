@@ -41,6 +41,9 @@ SIGNATURES = {
     "xfeat_mnn_presplit_workspace_bytes": (c_sz, [c_i, c_i, c_i]),
     "xfeat_mnn_match_presplit": (c_i, [c_p, c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_gather_matches": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_i, c_p, c_p, c_p]),
+    "xfeat_mnn_pairs_workspace_bytes": (c_sz, [c_i, c_i]),
+    "xfeat_mnn_match_pairs": (c_i, [c_p, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_gather_matches_pairs": (c_i, [c_p, c_i, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p]),
     "xfeat_refine_workspace_bytes": (c_sz, [c_i, c_i]),
     "xfeat_refine": (c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_kpts_heatmap": (c_i, [c_p, c_i, c_i, c_i, c_f, c_p, c_p]),

@@ -142,6 +142,9 @@ __global__ void __launch_bounds__(MNN_THREADS) mnn_scan_kernel(const float* __re
 // One CTA per pair: mutual test + threshold + ordered compaction.
 // f1 / f2 (optional, with their per-pair strides in floats): when given, the min_cossim test uses the fp32 dot product of the
 // matched rows instead of the packed value (implementation 4 carries approximate values for rows it did not re-score).
+// kPairs: pair p = (image i, image j) of `pairs` reads its counts as n1p[i], n2p[j] (the pair table of mnn_tc_kernel); row_best,
+// col_best and the outputs stay per pair.  A template flag, so that the per-pair instantiation keeps its code as it was.
+template <bool kPairs = false>
 __global__ void __launch_bounds__(1024) mnn_finalize_kernel(const unsigned long long* __restrict__ row_best,
                                                             const unsigned long long* __restrict__ col_best,
                                                             const int* __restrict__ n1p, const int* __restrict__ n2p,
@@ -150,12 +153,14 @@ __global__ void __launch_bounds__(1024) mnn_finalize_kernel(const unsigned long 
                                                             long long* __restrict__ idx0,
                                                             long long* __restrict__ idx1, int* __restrict__ n_matches,
                                                             const float* __restrict__ f1 = nullptr, int64_t stride1 = 0,
-                                                            const float* __restrict__ f2 = nullptr, int64_t stride2 = 0) {
+                                                            const float* __restrict__ f2 = nullptr, int64_t stride2 = 0,
+                                                            const int2* __restrict__ pairs = nullptr) {
   using Scan = cub::BlockScan<int, 1024>;
   __shared__ typename Scan::TempStorage tmp;
   __shared__ int s_base;
   const int pair = blockIdx.x;
-  const int n1 = n1p ? min(n1p[pair], n1_max) : n1_max;
+  const int2 ij = kPairs ? pairs[pair] : make_int2(pair, pair);
+  const int n1 = n1p ? min(n1p[ij.x], n1_max) : n1_max;
   if (threadIdx.x == 0) s_base = 0;
   const float vs = val_scale ? __ldg(val_scale) : 1.0f;   // tensor-core path carries values scaled by a power of two
   __syncthreads();
@@ -197,22 +202,25 @@ __global__ void __launch_bounds__(1024) mnn_finalize_kernel(const unsigned long 
     __syncthreads();
   }
   // a negative count is xfeat_detect_sparse's overflow indicator (XF_N_OVERFLOW): it propagates instead of reading as "no matches"
-  const bool overflow = (n1p && n1p[pair] < 0) || (n2p && n2p[pair] < 0);
+  const bool overflow = (n1p && n1p[ij.x] < 0) || (n2p && n2p[ij.y] < 0);
   if (threadIdx.x == 0) n_matches[pair] = overflow ? -1 : s_base;
 }
 
+// kPairs: pair p = (image i, image j) of `pairs` reads keypoints k0[i] and k1[j] (both usually the same image table)
+template <bool kPairs = false>
 __global__ void __launch_bounds__(256) gather_matches_kernel(const float* __restrict__ k0, const float* __restrict__ k1,
                                                              int n1_max, int n2_max, const long long* __restrict__ idx0,
                                                              const long long* __restrict__ idx1,
                                                              const int* __restrict__ n_matches, float* __restrict__ o0,
-                                                             float* __restrict__ o1) {
+                                                             float* __restrict__ o1, const int2* __restrict__ pairs = nullptr) {
   const int pair = blockIdx.y;
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= n_matches[pair]) return;
+  const int2 ij = kPairs ? __ldg(pairs + pair) : make_int2(pair, pair);
   const int64_t o = (int64_t)pair * n1_max + m;
   const long long a = idx0[o], b = idx1[o];
-  reinterpret_cast<float2*>(o0)[o] = __ldg(reinterpret_cast<const float2*>(k0) + (int64_t)pair * n1_max + a);
-  reinterpret_cast<float2*>(o1)[o] = __ldg(reinterpret_cast<const float2*>(k1) + (int64_t)pair * n2_max + b);
+  reinterpret_cast<float2*>(o0)[o] = __ldg(reinterpret_cast<const float2*>(k0) + (int64_t)ij.x * n1_max + a);
+  reinterpret_cast<float2*>(o1)[o] = __ldg(reinterpret_cast<const float2*>(k1) + (int64_t)ij.y * n2_max + b);
 }
 
 struct MnnWs {
@@ -242,7 +250,8 @@ static int g_mnn_impl = 1;
 size_t mnn_fast_workspace_bytes(int batch, int n1_max, int n2_max);
 int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const __half* f2s, const int* n2, int n2_max, int n_pad,
                            int batch, int scale_log2, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant);
+                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant,
+                           const int2* pairs = nullptr, int n_images = 0);
 int launch_mnn_fast(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                     int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
                     unsigned long long** best21, float** inv_s2, cudaStream_t st, float abs_bound, int sm_count);
@@ -350,6 +359,48 @@ extern "C" int xfeat_mnn_match_presplit(const void* d_f1s, const int32_t* d_n1, 
   if (rc) return rc;
   xf::mnn_finalize_kernel<<<batch, 1024, 0, st>>>(b12, b21, d_n1, d_n2, n1_max, n2_max, min_cossim, inv_s2, (long long*)d_idx0,
                                                   (long long*)d_idx1, d_n_matches);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" size_t xfeat_mnn_pairs_workspace_bytes(int n_pairs, int n_max) {
+  return xfeat_mnn_presplit_workspace_bytes(n_pairs, n_max, n_max);
+}
+
+extern "C" int xfeat_mnn_match_pairs(const void* d_fs, const int32_t* d_n, int n_images, int n_max, int n_pad,
+                                     const int32_t* d_pairs, int n_pairs, int scale_log2, float min_cossim, int64_t* d_idx0,
+                                     int64_t* d_idx1, int32_t* d_n_matches, void* d_ws, size_t ws_bytes, void* stream) {
+  XF_REQUIRE(d_fs && d_n && d_pairs && d_idx0 && d_idx1 && d_n_matches && d_ws, "mnn_match_pairs: null pointer");
+  XF_REQUIRE(n_images > 0 && n_pairs > 0 && n_pairs <= 65535 && n_max > 0, "mnn_match_pairs: bad sizes");
+  XF_REQUIRE(((uintptr_t)d_fs % 128) == 0, "mnn_match_pairs: operands must be 128-byte aligned");
+  XF_REQUIRE(((uintptr_t)d_pairs % 8) == 0, "mnn_match_pairs: the pair table must be 8-byte aligned");
+  if (xf::g_mnn_impl < 1 || xf::g_mnn_impl > 3) {
+    xf::set_error("mnn_match_pairs: implementation %d does not take pre-split operands (1, 2 and 3 do)", xf::g_mnn_impl);
+    return XF_E_UNSUPPORTED;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int2* pairs = reinterpret_cast<const int2*>(d_pairs);
+  unsigned long long *b12 = nullptr, *b21 = nullptr;
+  float* inv_s2 = nullptr;
+  int rc = xf::launch_mnn_tc_presplit((const __half*)d_fs, d_n, n_max, (const __half*)d_fs, d_n, n_max, n_pad, n_pairs, scale_log2,
+                                      d_ws, ws_bytes, &b12, &b21, &inv_s2, st, xf::g_mnn_impl - 1, pairs, n_images);
+  if (rc) return rc;
+  xf::mnn_finalize_kernel<true><<<n_pairs, 1024, 0, st>>>(b12, b21, d_n, d_n, n_max, n_max, min_cossim, inv_s2, (long long*)d_idx0,
+                                                    (long long*)d_idx1, d_n_matches, nullptr, 0, nullptr, 0, pairs);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" int xfeat_gather_matches_pairs(const float* d_kpts, int n_max, const int32_t* d_pairs, const int64_t* d_idx0,
+                                          const int64_t* d_idx1, const int32_t* d_n_matches, int n_pairs, float* d_out0,
+                                          float* d_out1, void* stream) {
+  XF_REQUIRE(d_kpts && d_pairs && d_idx0 && d_idx1 && d_n_matches && d_out0 && d_out1, "gather_matches_pairs: null pointer");
+  XF_REQUIRE(n_pairs > 0 && n_pairs <= 65535 && n_max > 0, "gather_matches_pairs: bad sizes");
+  XF_REQUIRE(((uintptr_t)d_pairs % 8) == 0, "gather_matches_pairs: the pair table must be 8-byte aligned");
+  dim3 grid(xf::cdiv(n_max, 256), n_pairs);
+  xf::gather_matches_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(d_kpts, d_kpts, n_max, n_max, (const long long*)d_idx0,
+                                                                    (const long long*)d_idx1, d_n_matches, d_out0, d_out1,
+                                                                    reinterpret_cast<const int2*>(d_pairs));
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -145,16 +145,21 @@ __device__ __forceinline__ void mnn_row_argmax(const float (&acc0)[64], const fl
 
 // rows_cnt (optional): [pair][dir] number of rows of the A array to scan (the compact lists of mnn_fast.cu) instead of the
 // set size; row_map (optional): [pair][dir][n_pad] output row of compact row r.
+// pairs (optional): pair p = (image i, image j) of one image table of n_images * n_pad rows that every map covers; the counts are
+// n1p[i] and n2p[j], the A rows of direction 0 start at i * n_pad and its B rows at j * n_pad (the other way round for direction 1).
+// best12 / best21 stay per pair.  NULL: image p of each set is pair p.
 __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_kernel(const __grid_constant__ TcMaps4 maps,
                                                                const int* __restrict__ n1p, int n1_max,
                                                                const int* __restrict__ n2p, int n2_max, int n_pad,
                                                                unsigned long long* __restrict__ best12,
                                                                unsigned long long* __restrict__ best21,
                                                                const int* __restrict__ rows_cnt,
-                                                               const int* __restrict__ row_map) {
+                                                               const int* __restrict__ row_map,
+                                                               const int2* __restrict__ pairs) {
   const int pair = blockIdx.y, dir = blockIdx.z;
-  const int n1 = n1p ? min(n1p[pair], n1_max) : n1_max;
-  const int n2 = n2p ? min(n2p[pair], n2_max) : n2_max;
+  const int2 ij = pairs ? __ldg(pairs + pair) : make_int2(pair, pair);
+  const int n1 = n1p ? min(n1p[ij.x], n1_max) : n1_max;
+  const int n2 = n2p ? min(n2p[ij.y], n2_max) : n2_max;
   const int n_rows = rows_cnt ? min(rows_cnt[pair * 2 + dir], n_pad) : (dir ? n2 : n1), n_cols = dir ? n1 : n2;
   const int out_stride = dir ? n2_max : n1_max;
   unsigned long long* out = dir ? best21 : best12;
@@ -190,12 +195,12 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_kernel(const __grid_cons
   if (warp == 8) {
     if (T > 0 && tc::elect_one()) {
       // ---------------- TMA producer ----------------
-      const int arow = pair * n_pad + row0;
+      const int arow = (dir ? ij.y : ij.x) * n_pad + row0;
       tc::mbar_expect_tx(a_full, 4 * TC_BOX_BYTES);
       for (int slab = 0; slab < 2; ++slab)
         for (int kb = 0; kb < 2; ++kb)
           tc::tma_load_2d(sA + (slab * 2 + kb) * TC_BOX_BYTES, mapA, a_full, kb * 64, arow + slab * 128);
-      const int brow = pair * n_pad;
+      const int brow = (dir ? ij.x : ij.y) * n_pad;
       for (int t = 0; t < T; ++t) {
         const int s = t & 1;
         tc::mbar_wait(&b_empty[s], ((t >> 1) & 1) ^ 1);
@@ -247,7 +252,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __
                                                                        const int* __restrict__ n1p, int n1_max,
                                                                        const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
                                                                        unsigned long long* __restrict__ best12,
-                                                                       unsigned long long* __restrict__ best21) {
+                                                                       unsigned long long* __restrict__ best21,
+                                                                       const int2* __restrict__ pairs) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sA = base;                       // [buffer 2][slab 2][hi, lo] boxes
@@ -277,16 +283,20 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __
   }
   __syncthreads();
 
-  // item -> (pair, dir, row block); every role walks the same sequence and skips the same (empty) items
-  auto decode = [&](int item, int& pair, int& dir, int& row0, int& n_rows, int& n_cols) {
+  // item -> (pair, dir, row block) and the images (ia, ib) of its A and B rows (pairs: see mnn_tc_kernel); every role walks the
+  // same sequence and skips the same (empty) items
+  auto decode = [&](int item, int& pair, int& dir, int& row0, int& n_rows, int& n_cols, int& ia, int& ib) {
     const int rb = item % RB, pd = item / RB;
     pair = pd >> 1;
     dir = pd & 1;
     row0 = rb * TC_ROWS;
-    const int n1 = n1p ? min(__ldg(n1p + pair), n1_max) : n1_max;
-    const int n2 = n2p ? min(__ldg(n2p + pair), n2_max) : n2_max;
+    const int2 ij = pairs ? __ldg(pairs + pair) : make_int2(pair, pair);
+    const int n1 = n1p ? min(__ldg(n1p + ij.x), n1_max) : n1_max;
+    const int n2 = n2p ? min(__ldg(n2p + ij.y), n2_max) : n2_max;
     n_rows = dir ? n2 : n1;
     n_cols = dir ? n1 : n2;
+    ia = dir ? ij.y : ij.x;
+    ib = dir ? ij.x : ij.y;
     return row0 < n_rows && n_cols > 0;
   };
 
@@ -294,20 +304,20 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __
     if (tc::elect_one()) {
       uint32_t ai = 0, bi = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int pair, dir, row0, n_rows, n_cols;
-        if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
+        int pair, dir, row0, n_rows, n_cols, ia, ib;
+        if (!decode(item, pair, dir, row0, n_rows, n_cols, ia, ib)) continue;
         const CUtensorMap* mapA = dir ? &maps.m2 : &maps.m1;
         const CUtensorMap* mapB = dir ? &maps.m1 : &maps.m2;
         const int T = (n_cols + TC_BN - 1) / TC_BN;
         const int ab = ai & 1;
         tc::mbar_wait(&a_empty[ab], ((ai >> 1) & 1) ^ 1);
         tc::mbar_expect_tx(&a_full[ab], 4 * TC_BOX_BYTES);
-        const int arow = pair * n_pad + row0;
+        const int arow = ia * n_pad + row0;
         for (int slab = 0; slab < 2; ++slab)
           for (int kb = 0; kb < 2; ++kb)
             tc::tma_load_2d(sA + ((ab * 2 + slab) * 2 + kb) * TC_BOX_BYTES, mapA, &a_full[ab], kb * 64, arow + slab * 128);
         ++ai;
-        const int brow = pair * n_pad;
+        const int brow = ib * n_pad;
         for (int t = 0; t < T; ++t, ++bi) {
           const int s = bi % TCP_NSB;
           tc::mbar_wait(&b_empty[s], ((bi / TCP_NSB) & 1) ^ 1);
@@ -323,8 +333,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __
     float acc0[64], acc1[64];
     uint32_t ai = 0, bi = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      int pair, dir, row0, n_rows, n_cols;
-      if (!decode(item, pair, dir, row0, n_rows, n_cols)) continue;
+      int pair, dir, row0, n_rows, n_cols, ia, ib;
+      if (!decode(item, pair, dir, row0, n_rows, n_cols, ia, ib)) continue;
       const int T = (n_cols + TC_BN - 1) / TC_BN;
       const int ab = ai & 1;
       tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
@@ -454,7 +464,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
                                                                        const int* __restrict__ n1p, int n1_max,
                                                                        const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
                                                                        unsigned long long* __restrict__ best12,
-                                                                       unsigned long long* __restrict__ best21) {
+                                                                       unsigned long long* __restrict__ best21,
+                                                                       const int2* __restrict__ pairs) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* sA = base;                       // [buffer 2][slab 2][hi, lo] boxes
@@ -485,12 +496,16 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
   }
   __syncthreads();
 
-  // item -> (pair, row block); every role walks the same sequence and skips the same (empty) items
-  auto decode = [&](int item, int& pair, int& row0, int& n_rows, int& n_cols) {
+  // item -> (pair, row block) and the images (ia, ib) of its A and B rows (pairs: see mnn_tc_kernel); every role walks the same
+  // sequence and skips the same (empty) items
+  auto decode = [&](int item, int& pair, int& row0, int& n_rows, int& n_cols, int& ia, int& ib) {
     pair = item / RB;
     row0 = (item - pair * RB) * TC_ROWS;
-    n_rows = n1p ? min(__ldg(n1p + pair), n1_max) : n1_max;
-    n_cols = n2p ? min(__ldg(n2p + pair), n2_max) : n2_max;
+    const int2 ij = pairs ? __ldg(pairs + pair) : make_int2(pair, pair);
+    ia = ij.x;
+    ib = ij.y;
+    n_rows = n1p ? min(__ldg(n1p + ia), n1_max) : n1_max;
+    n_cols = n2p ? min(__ldg(n2p + ib), n2_max) : n2_max;
     return row0 < n_rows && n_cols > 0;
   };
 
@@ -498,18 +513,18 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
     if (tc::elect_one()) {
       uint32_t ai = 0, bi = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int pair, row0, n_rows, n_cols;
-        if (!decode(item, pair, row0, n_rows, n_cols)) continue;
+        int pair, row0, n_rows, n_cols, ia, ib;
+        if (!decode(item, pair, row0, n_rows, n_cols, ia, ib)) continue;
         const int T = (n_cols + TC_BN - 1) / TC_BN;
         const int ab = ai & 1;
         tc::mbar_wait(&a_empty[ab], ((ai >> 1) & 1) ^ 1);
         tc::mbar_expect_tx(&a_full[ab], 4 * TC_BOX_BYTES);
-        const int arow = pair * n_pad + row0;
+        const int arow = ia * n_pad + row0;
         for (int slab = 0; slab < 2; ++slab)
           for (int kb = 0; kb < 2; ++kb)
             tc::tma_load_2d(sA + ((ab * 2 + slab) * 2 + kb) * TC_BOX_BYTES, &maps.m1, &a_full[ab], kb * 64, arow + slab * 128);
         ++ai;
-        const int brow = pair * n_pad;
+        const int brow = ib * n_pad;
         for (int t = 0; t < T; ++t, ++bi) {
           const int s = bi % TCF_NSB;
           tc::mbar_wait(&b_empty[s], ((bi / TCF_NSB) & 1) ^ 1);
@@ -527,8 +542,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
     uint32_t ai = 0, bi = 0;
     if (slab == 1) named_arrive(1, 256);   // warpgroup 0 goes first
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      int pair, row0, n_rows, n_cols;
-      if (!decode(item, pair, row0, n_rows, n_cols)) continue;
+      int pair, row0, n_rows, n_cols, ia, ib;
+      if (!decode(item, pair, row0, n_rows, n_cols, ia, ib)) continue;
       const int T = (n_cols + TC_BN - 1) / TC_BN;
       const int ab = ai & 1;
       const int srow0 = row0 + slab * 128;
@@ -603,16 +618,17 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
 
 // The three-term scan of both directions over the full sets.  variant 0 (implementation 1, default): the single-GEMM persistent
 // kernel; 1 (implementation 2): the persistent kernel with one GEMM per direction; 2 (implementation 3) or XFEAT_MNN_ONESHOT=1:
-// one CTA per (row block, pair, direction).
+// one CTA per (row block, pair, direction).  pairs: optional (image i, image j) table (see mnn_tc_kernel).
 static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, const int* n2, int n2_max, int n_pad, int batch,
-                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st, int variant) {
+                              unsigned long long* best12, unsigned long long* best21, cudaStream_t st, int variant,
+                              const int2* pairs = nullptr) {
   static const bool oneshot_env = getenv("XFEAT_MNN_ONESHOT") != nullptr;
   if (variant == 2 || oneshot_env) {
     XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
     dim3 grid(n_pad / TC_ROWS, batch, 2);
     TcMaps4 m4;
     m4.a0 = maps.m1; m4.b0 = maps.m2; m4.a1 = maps.m2; m4.b1 = maps.m1;
-    mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, nullptr, nullptr);
+    mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, nullptr, nullptr, pairs);
     XF_LAUNCH_CHECK();
     return XF_OK;
   }
@@ -623,12 +639,12 @@ static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, con
     XF_DYN_SMEM(mnn_tc_persist2_kernel, TCP_SMEM);
     const int n_items = batch * 2 * (n_pad / TC_ROWS);
     mnn_tc_persist2_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCP_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
-                                                                                       best12, best21);
+                                                                                       best12, best21, pairs);
   } else {
     XF_DYN_SMEM(mnn_tc_persist_kernel, TCF_SMEM);
     const int n_items = batch * (n_pad / TC_ROWS);
     mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCF_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
-                                                                                      best12, best21);
+                                                                                      best12, best21, pairs);
   }
   XF_LAUNCH_CHECK();
   return XF_OK;
@@ -721,11 +737,15 @@ int launch_mnn_tc_rows(const __half* a0, const __half* b0, const __half* a1, con
 __global__ void set_scalar_kernel(float* p, float v) { *p = v; }
 
 // Operands already split by the producer (xfeat_detect_sparse_split): (batch * n_pad) rows x 128 halves each, scaled by 2^scale_log2.
+// pairs != NULL: f1s == f2s is one table of n_images images (n_images * n_pad rows) and pair p matches the images pairs[p] = (i, j)
+// of it (the counts n1[i], n2[j]); batch is the number of pairs.
 int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const __half* f2s, const int* n2, int n2_max, int n_pad,
                            int batch, int scale_log2, void* d_ws, size_t ws_bytes, unsigned long long** best12,
-                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant) {
+                           unsigned long long** best21, float** inv_s2, cudaStream_t st, int variant,
+                           const int2* pairs, int n_images) {
   XF_REQUIRE(n_pad % (2 * TC_ROWS) == 0 && n_pad >= n1_max && n_pad >= n2_max, "mnn_match_presplit: n_pad must be a multiple of %d covering both sets", 2 * TC_ROWS);
-  XF_REQUIRE((int64_t)batch * n_pad < (1ll << 31), "mnn_match_presplit: batch * n too large");
+  const int64_t table_rows = (int64_t)(pairs ? n_images : batch) * n_pad;
+  XF_REQUIRE(table_rows < (1ll << 31), "mnn_match_presplit: batch * n too large");
   Bump bump(d_ws, ws_bytes);
   unsigned long long* b12 = bump.take<unsigned long long>((size_t)batch * n1_max);
   unsigned long long* b21 = bump.take<unsigned long long>((size_t)batch * n2_max);
@@ -741,9 +761,9 @@ int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const _
   *best12 = b12; *best21 = b21; *inv_s2 = scale;
   TcMaps maps;
   int rc;
-  if ((rc = make_map(&maps.m1, f1s, (uint64_t)batch * n_pad))) return rc;
-  if ((rc = make_map(&maps.m2, f2s, (uint64_t)batch * n_pad))) return rc;
-  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, variant);
+  if ((rc = make_map(&maps.m1, f1s, (uint64_t)table_rows))) return rc;
+  if ((rc = make_map(&maps.m2, f2s, (uint64_t)table_rows))) return rc;
+  return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, variant, pairs);
 }
 
 int launch_absmax(const float* f, const int* np, int n_max, int64_t stride, int batch, unsigned* out, cudaStream_t st) {
@@ -766,7 +786,7 @@ int launch_mnn_tc_rows(const __half* a0, const __half* b0, const __half* a1, con
   if ((rc = make_map(&m4.b1, b1, (uint64_t)batch * n_pad))) return rc;
   XF_DYN_SMEM(mnn_tc_kernel, TC_SMEM);
   dim3 grid(n_pad / TC_ROWS, batch, 2);
-  mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, rows_cnt, row_map);
+  mnn_tc_kernel<<<grid, MT_THREADS, TC_SMEM, st>>>(m4, n1, n1_max, n2, n2_max, n_pad, best12, best21, rows_cnt, row_map, nullptr);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

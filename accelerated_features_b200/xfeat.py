@@ -7,7 +7,8 @@ There is no CPU / eager fallback: without a CUDA device and the built library th
 
 Beyond the reference surface: `match_xfeat_batch` (batched match_xfeat) and `match_xfeat_stream` (pinned, double-buffered
 host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match_lighterglue_batch` and
-`match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu).
+`match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu), `match_xfeat_pairs` and
+`match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once).
 """
 from __future__ import annotations
 
@@ -28,6 +29,74 @@ _D2H_ON_MAIN = bool(os.environ.get("XFEAT_STREAM_D2H_MAIN"))   # A/B switch of m
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# host-side plan of match_xfeat_pairs (no device work: testable without a GPU)
+# ----------------------------------------------------------------------------------------------------------------------
+PAIRS_EXTRACT_CHUNK = 64      # images per extraction launch sequence
+PAIRS_MATCH_CHUNK = 4096      # pairs per matcher launch (and per host synchronisation)
+
+
+def pair_image_key(x) -> tuple:
+    """Extraction bucket of one image of match_xfeat_pairs: (C, H, W, dtype, div255), with the dtype and the "/255" flag that
+    _parse_input gives it (numpy uint8: "/255" on the device; numpy float: divided on the host, float32; tensors: as they are).
+    numpy (H,W) is read as (H,W,1); tensors are (C,H,W) or (1,C,H,W)."""
+    if isinstance(x, np.ndarray):
+        if x.ndim == 2:
+            return (1, x.shape[0], x.shape[1], "uint8" if x.dtype == np.uint8 else "float32", x.dtype == np.uint8)
+        if x.ndim == 3:
+            return (x.shape[2], x.shape[0], x.shape[1], "uint8" if x.dtype == np.uint8 else "float32", x.dtype == np.uint8)
+        raise RuntimeError("match_xfeat_pairs: numpy images must be (H,W) or (H,W,C)")
+    if isinstance(x, torch.Tensor):
+        if x.ndim == 4 and x.shape[0] == 1:
+            x = x[0]
+        if x.ndim != 3:
+            raise RuntimeError("match_xfeat_pairs: tensor images must be (C,H,W) or (1,C,H,W)")
+        return (x.shape[0], x.shape[1], x.shape[2], str(x.dtype).replace("torch.", ""), False)
+    raise RuntimeError(f"match_xfeat_pairs: unsupported image type {type(x).__name__}")
+
+
+def check_pairs(pairs, n_images: int) -> np.ndarray:
+    """`pairs` as a validated (P, 2) int64 array of indices into `n_images` images (P = 0 for an empty input)."""
+    a = np.asarray(pairs)
+    if a.size == 0:
+        return np.zeros((0, 2), np.int64)
+    if a.ndim != 2 or a.shape[1] != 2:
+        raise ValueError(f"pairs must be (P, 2), got shape {a.shape}")
+    if not np.issubdtype(a.dtype, np.integer):
+        raise TypeError(f"pairs must hold integers, got {a.dtype}")
+    if a.min() < 0 or a.max() >= n_images:
+        bad = np.nonzero((a < 0).any(1) | (a >= n_images).any(1))[0]
+        raise ValueError(f"pairs {bad[:8].tolist()} index outside the {n_images} images")
+    return a.astype(np.int64)
+
+
+class PairPlan:
+    """Which images match_xfeat_pairs extracts, where their rows go and how the pairs address them.
+
+    chunks: lists of image indices; each list shares one bucket key and is at most `chunk` long.  Table slots are assigned in
+    chunk order (chunk 0 takes slots 0..len-1, ...), so slot[image] is the image's row in the keypoint / operand tables (-1:
+    no pair references it, not extracted).  table_pairs (P, 2) int32: the pairs in slot numbers."""
+
+    def __init__(self, keys, pairs, chunk: int = PAIRS_EXTRACT_CHUNK):
+        self.pairs = check_pairs(pairs, len(keys))
+        used = np.zeros(len(keys), bool)
+        used[self.pairs.ravel()] = True
+        buckets: Dict[tuple, List[int]] = {}
+        for n in np.nonzero(used)[0].tolist():
+            buckets.setdefault(keys[n], []).append(n)
+        self.chunks = [b[o:o + chunk] for b in buckets.values() for o in range(0, len(b), chunk)]
+        self.slot = np.full(len(keys), -1, np.int64)
+        order = [n for c in self.chunks for n in c]
+        self.slot[order] = np.arange(len(order))
+        self.n_slots = len(order)
+        self.table_pairs = self.slot[self.pairs].astype(np.int32).reshape(-1, 2)
+
+    def match_order(self) -> np.ndarray:
+        """Order in which the pairs are matched: by (j, i) of the table pairs, so that the pairs running at the same time stream
+        the same second image (its rows stay in L2)."""
+        return np.lexsort((self.table_pairs[:, 0], self.table_pairs[:, 1]))
 
 
 class InterpolateSparse2d(torch.nn.Module):
@@ -201,11 +270,13 @@ class XFeat(torch.nn.Module):
         return x, 0
 
     @staticmethod
-    def _check_counts(counts: List[int], what: str):
+    def _check_counts(counts: List[int], what: str, labels: Optional[List[str]] = None):
+        """`labels`: how to name item b in the error (default: "batch items [b, ...]")."""
         if counts and min(counts) < 0:
             bad = [i for i, c in enumerate(counts) if c < 0]
+            items = f"batch items {bad}" if labels is None else ", ".join(labels[i] for i in bad)
             raise _lib.XFeatLibraryError(
-                f"{what}: NMS candidate buffer overflow (more than H*W/4 maxima above the threshold) for batch items {bad}; "
+                f"{what}: NMS candidate buffer overflow (more than H*W/4 maxima above the threshold) for {items}; "
                 "nothing is returned for them rather than an arbitrary subset")
 
     def _preprocess(self, x: torch.Tensor, H: int, W: int, div255: bool, out: Optional[torch.Tensor] = None,
@@ -262,11 +333,13 @@ class XFeat(torch.nn.Module):
         return (top_k + 511) // 512 * 512                       # row padding of the tensor-core matcher (mnn_tc.cu)
 
     def _detect_sparse_device(self, x, top_k: int, detection_threshold: float, div255=False, want_split: bool = False,
-                              want_desc: bool = True):
+                              want_desc: bool = True, out: Optional[Dict[str, torch.Tensor]] = None):
         """Whole sparse extraction on the device, fixed-capacity outputs, no host sync.  `x` is one image batch or a list
         of batches of identical shape (they are normalised into one activation batch without concatenating the inputs);
         `div255` is one flag or one per batch (parse_input's "/255" applies to numpy inputs only, xfeat.py:400-401).
         `want_split`: also return 'desc_split' (B, split_rows, 128) fp16, the matcher's pre-split operand rows.
+        `out`: write 'keypoints', 'n_valid' and (when asked for) 'descriptors' / 'desc_split' into these (B, ...) tensors, e.g.
+        slices of an image table, instead of fresh ones.
         Returns dict of device tensors: keypoints (B,k,2), scores (B,k), descriptors (B,k,64), n_valid (B) int32."""
         xs = [self._to_bchw(t) for t in (x if isinstance(x, (list, tuple)) else [x])]
         flags = list(div255) if isinstance(div255, (list, tuple)) else [div255] * len(xs)
@@ -288,17 +361,22 @@ class XFeat(torch.nn.Module):
             self._preprocess(t, H, W, bool(f), out=xn[o:o + t.shape[0]])
             o += t.shape[0]
         feats, heat, rel, _ = self._run_net(xn, B, H, W)
-        kpts = self._empty((B, top_k, 2))
+        dst = out or {}
+        kpts = dst["keypoints"] if "keypoints" in dst else self._empty((B, top_k, 2))
         scores = self._empty((B, top_k))
-        desc = self._empty((B, top_k, 64)) if (want_desc or not want_split) else None   # match-only callers take the split rows alone
-        n_valid = self._empty((B,), torch.int32)
+        desc = None
+        if want_desc or not want_split:                     # match-only callers take the split rows alone
+            desc = dst["descriptors"] if "descriptors" in dst else self._empty((B, top_k, 64))
+        n_valid = dst["n_valid"] if "n_valid" in dst else self._empty((B,), torch.int32)
         n_cand = self._empty((B,), torch.int32)
         nbytes = self._lib.xfeat_sparse_workspace_bytes(B, H, W, top_k)
         if nbytes == 0:
             raise _lib.XFeatLibraryError("xfeat_sparse_workspace_bytes failed: " + self._lib.xfeat_last_error().decode())
         ws = self._workspace(nbytes)
         split_rows = self._split_rows(top_k)
-        split = self._empty((B, split_rows, 128), torch.float16) if want_split else None
+        split = None
+        if want_split:
+            split = dst["desc_split"] if "desc_split" in dst else self._empty((B, split_rows, 128), torch.float16)
         with torch.cuda.device(self.dev):
             _lib.check(self._lib.xfeat_detect_sparse_split(self._ctx, feats.data_ptr(), heat.data_ptr(), rel.data_ptr(), B, H, W,
                                                            top_k, float(detection_threshold), float(_F32(rw)), float(_F32(rh)),
@@ -500,24 +578,25 @@ class XFeat(torch.nn.Module):
             raise RuntimeError("Input tensor needs to be in (B,C,H,W) format")
         return x, False, False
 
-    def _upload(self, pipe, slot: int, pair):
-        """Queue the H2D copies of one batch on the copy stream (into the slot's device buffers)."""
-        hs = [self._host_batch(pair[0]), self._host_batch(pair[1])]
+    def _upload(self, pipe, slot: int, batches):
+        """Queue the H2D copies of a list of image batches on the copy stream (into the slot's device buffers): the two image
+        sets of one match_xfeat_stream batch, or the images of one match_xfeat_pairs chunk."""
+        hs = [self._host_batch(b) for b in batches]
         devs, stages = [], []
-        prev_dev = pipe.dev_in[slot] or [None, None]
-        prev_stage = pipe.stage[slot] or [None, None]
+        prev_dev = pipe.dev_in[slot] or []
+        prev_stage = pipe.stage[slot] or []
         for j, (t, _, _) in enumerate(hs):          # device slots come from the compute stream's pool (they are read there)
             if t.is_cuda:
                 devs.append(t)
                 continue
-            old = prev_dev[j]
+            old = prev_dev[j] if j < len(prev_dev) else None
             if old is None or old.shape != t.shape or old.dtype != t.dtype or old.data_ptr() == t.data_ptr():
                 old = torch.empty(t.shape, dtype=t.dtype, device=self.dev)
             devs.append(old)
         for j, (t, _, _) in enumerate(hs):
             st = None
             if not t.is_cuda and not t.is_pinned():
-                st = prev_stage[j]
+                st = prev_stage[j] if j < len(prev_stage) else None
                 if st is None or st.shape != t.shape or st.dtype != t.dtype:
                     st = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
                 else:
@@ -603,6 +682,149 @@ class XFeat(torch.nn.Module):
             i += 1
         if pending is not None:
             yield finish(pending)
+
+    # ------------------------------------------------------------------------------------------------------------
+    # pair lists over a shared set of images: every referenced image is extracted once
+    # ------------------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _pair_image(x):
+        """One image of match_xfeat_pairs as _host_batch takes it (numpy (H,W) -> (H,W,1))."""
+        return x[:, :, None] if isinstance(x, np.ndarray) and x.ndim == 2 else x
+
+    def _extract_table(self, images, plan: PairPlan, top_k: int, want_split: bool, want_desc: bool) -> Dict[str, torch.Tensor]:
+        """Sparse extraction of every planned image into one table (row = slot): keypoints (n, top_k, 2), n_valid (n) and the
+        descriptors (n, top_k, 64) and / or operand rows (n, split_rows, 128).  The chunks go through match_xfeat_stream's copy
+        pipeline: chunk c+1 is uploaded on the copy stream while chunk c is extracted.  No host sync."""
+        n = plan.n_slots
+        tab = {"keypoints": self._empty((n, top_k, 2)), "n_valid": self._empty((n,), torch.int32)}
+        if want_desc:
+            tab["descriptors"] = self._empty((n, top_k, 64))
+        if want_split:
+            tab["desc_split"] = self._empty((n, self._split_rows(top_k), 128), torch.float16)
+        if self._pipe is None:
+            self._pipe = XFeat._Pipe(self.dev)
+        pipe = self._pipe
+        main = torch.cuda.current_stream(self.dev)
+        for ev in pipe.freed:
+            ev.record(main)
+
+        def upload(c: int, slot: int):
+            return self._upload(pipe, slot, [self._pair_image(images[i]) for i in plan.chunks[c]])
+
+        cur, s0 = upload(0, 0), 0
+        for c, chunk in enumerate(plan.chunks):
+            slot = c & 1
+            nxt = upload(c + 1, slot ^ 1) if c + 1 < len(plan.chunks) else None     # overlaps the kernels queued below
+            main.wait_event(pipe.ready[slot])
+            s1 = s0 + len(chunk)
+            self._detect_sparse_device([x for x, _ in cur], top_k, self.detection_threshold, [f for _, f in cur],
+                                       want_split=want_split, want_desc=want_desc, out={k: v[s0:s1] for k, v in tab.items()})
+            pipe.freed[slot].record(main)
+            cur, s0 = nxt, s1
+        return tab
+
+    def _mnn_pairs_device(self, tab, tp: torch.Tensor, top_k: int, min_cossim: float):
+        """xfeat_mnn_match_pairs on the table's operand rows for the (B, 2) int32 device pair table `tp`."""
+        B = tp.shape[0]
+        sp = tab["desc_split"]
+        idx0 = self._empty((B, top_k), torch.int64)
+        idx1 = self._empty((B, top_k), torch.int64)
+        cnt = self._empty((B,), torch.int32)
+        ws = self._workspace(self._lib.xfeat_mnn_pairs_workspace_bytes(B, top_k))
+        with torch.cuda.device(self.dev):
+            _lib.check(self._lib.xfeat_mnn_match_pairs(sp.data_ptr(), tab["n_valid"].data_ptr(), sp.shape[0], top_k, sp.shape[1],
+                                                       tp.data_ptr(), B, 13, float(min_cossim), idx0.data_ptr(), idx1.data_ptr(),
+                                                       cnt.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()),
+                       "xfeat_mnn_match_pairs")
+        return idx0, idx1, cnt
+
+    @staticmethod
+    def _pair_labels(plan: PairPlan, sel: np.ndarray) -> List[str]:
+        return [f"pair {p} (images {plan.pairs[p, 0]}, {plan.pairs[p, 1]})" for p in sel.tolist()]
+
+    @torch.inference_mode()
+    def match_xfeat_pairs(self, images, pairs, top_k=None, min_cossim=-1) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """match_xfeat over a list of pairs into one set of images: result p is what match_xfeat(images[i], images[j], top_k,
+        min_cossim) returns for pairs[p] = (i, j), bit for bit -- self pairs, repeated pairs and both orders included.
+
+        images: sequence of single images in any mix of shapes and types -- numpy (H,W) / (H,W,C), uint8 or float, or torch
+        (C,H,W) / (1,C,H,W) on the host or the device (numpy (H,W) is read as (H,W,1)).  pairs: (P, 2) array-like of ints.
+        Only images some pair names are extracted, each exactly once, in launch sequences of up to 64 images of one
+        (C, H, W, dtype, "/255") bucket; the pairs are then matched straight from the shared table, up to 4096 per launch."""
+        if top_k is None: top_k = self.top_k
+        plan = PairPlan([pair_image_key(x) for x in images], pairs)
+        if len(plan.pairs) == 0:
+            return []
+        presplit = self._lib.xfeat_get_mnn_impl() in (1, 2, 3)   # else: fp32 descriptors, per-pair gather, xfeat_mnn_match_bounded
+        order = plan.match_order()
+        tp_all = torch.from_numpy(np.ascontiguousarray(plan.table_pairs[order])).to(self.dev)
+        tab = self._extract_table(images, plan, top_k, want_split=presplit, want_desc=not presplit)
+        out: List = [None] * len(order)
+        step = PAIRS_MATCH_CHUNK if presplit else 256              # the fp32 fallback gathers (B, top_k, 64) per side
+        for o in range(0, len(order), step):
+            sel, tp = order[o:o + step], tp_all[o:o + step]
+            B = len(sel)
+            if presplit:
+                idx0, idx1, cnt = self._mnn_pairs_device(tab, tp, top_k, min_cossim)
+            else:
+                ti, tj = tp[:, 0].long(), tp[:, 1].long()
+                d, n = tab["descriptors"], tab["n_valid"]
+                idx0, idx1, cnt = self._mnn_device(d.index_select(0, ti), n.index_select(0, ti), top_k, top_k * 64,
+                                                   d.index_select(0, tj), n.index_select(0, tj), top_k, top_k * 64, B, min_cossim,
+                                                   abs_bound=1.0)
+            mk0, mk1 = self._empty((B, top_k, 2)), self._empty((B, top_k, 2))
+            with torch.cuda.device(self.dev):
+                _lib.check(self._lib.xfeat_gather_matches_pairs(tab["keypoints"].data_ptr(), top_k, tp.data_ptr(), idx0.data_ptr(),
+                                                                idx1.data_ptr(), cnt.data_ptr(), B, mk0.data_ptr(),
+                                                                mk1.data_ptr(), self._stream()), "xfeat_gather_matches_pairs")
+            h0, h1 = (torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (mk0, mk1))
+            hc = torch.empty((B,), dtype=torch.int32, pin_memory=True)
+            for h, t in ((h0, mk0), (h1, mk1), (hc, cnt)):
+                h.copy_(t, non_blocking=True)
+            torch.cuda.current_stream(self.dev).synchronize()         # the only host sync of this chunk
+            c = hc.tolist()
+            self._check_counts(c, "match_xfeat_pairs", self._pair_labels(plan, sel))
+            a0, a1 = h0.numpy(), h1.numpy()
+            for b, p in enumerate(sel.tolist()):
+                out[p] = (a0[b, :c[b]].copy(), a1[b, :c[b]].copy())
+        return out
+
+    @torch.inference_mode()
+    def match_xfeat_lighterglue_pairs(self, images, pairs, top_k=None, min_conf: float = 0.1,
+                                      prune_min_points: Optional[int] = LG_PRUNE_MIN_POINTS) -> List[Tuple[np.ndarray, np.ndarray, np.ndarray]]:
+        """match_xfeat_lighterglue_batch over a list of pairs into one set of images (inputs as match_xfeat_pairs): result p equals
+        match_xfeat_lighterglue_batch on (images[i], images[j]) alone.  Each referenced image is extracted once; the pairs' sides
+        are gathered from the table on the device, up to 256 pairs per LighterGlue launch."""
+        if top_k is None: top_k = self.top_k
+        keys = [pair_image_key(x) for x in images]
+        plan = PairPlan(keys, pairs)
+        if len(plan.pairs) == 0:
+            return []
+        self._lg()                                                  # weights load before any extraction is queued
+        tab = self._extract_table(images, plan, top_k, want_split=False, want_desc=True)
+        used = np.nonzero(plan.slot >= 0)[0]
+        sizes = np.zeros((plan.n_slots, 2), np.float32)
+        sizes[plan.slot[used]] = [(keys[i][2], keys[i][1]) for i in used]            # (W, H) of the image as given
+        sizes = torch.from_numpy(sizes).to(self.dev)
+        out: List = [None] * len(plan.pairs)
+        step = 256
+        for o in range(0, len(plan.pairs), step):
+            sel = np.arange(o, min(o + step, len(plan.pairs)))
+            tp = torch.from_numpy(plan.table_pairs[sel].astype(np.int64)).to(self.dev)
+            side = [{k: tab[k].index_select(0, tp[:, s]) for k in ("keypoints", "descriptors", "n_valid")} for s in (0, 1)]
+            s0, s1 = sizes.index_select(0, tp[:, 0]), sizes.index_select(0, tp[:, 1])
+            k0, k1 = side[0]["keypoints"], side[1]["keypoints"]
+            idx0, idx1, _, cnt = self.match_lighterglue_batch(k0, side[0]["descriptors"], side[0]["n_valid"], s0, k1,
+                                                              side[1]["descriptors"], side[1]["n_valid"], s1, min_conf,
+                                                              prune_min_points)
+            B = len(sel)
+            mk0, mk1, cnt = self._gather_matches(k0, k1, idx0, idx1, cnt, B, top_k)
+            c = cnt.tolist()
+            self._check_counts(c, "match_xfeat_lighterglue_pairs", self._pair_labels(plan, sel))
+            mk0, mk1, i0, i1 = (t.cpu().numpy() for t in (mk0, mk1, idx0, idx1))
+            for b, p in enumerate(sel.tolist()):
+                out[p] = (mk0[b, :c[b]], mk1[b, :c[b]], np.stack([i0[b, :c[b]], i1[b, :c[b]]], -1))
+        return out
 
     # ------------------------------------------------------------------------------------------------------------
     # semi-dense path

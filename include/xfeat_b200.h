@@ -189,6 +189,21 @@ XF_API int xfeat_gather_matches(const float* d_kpts0, const float* d_kpts1, int 
                          const int64_t* d_idx0, const int64_t* d_idx1, const int32_t* d_n_matches, int batch,
                          float* d_out0, float* d_out1, void* stream);
 
+/* Pair lists over one image table (XFeat.match_xfeat_pairs): each image's operand rows are written once and matched in every
+ * pair that names it.  d_fs (n_images, n_pad, 128) fp16 [hi|lo] rows as xfeat_detect_sparse_split writes them (scale
+ * 2^scale_log2), d_n (n_images) counts, d_pairs (n_pairs, 2) int32 device image indices, each in [0, n_images) (the caller
+ * validates them).  Outputs per pair p at capacity n_max, identical to xfeat_mnn_match_presplit on images (i, j) alone; a pair
+ * with an XF_N_OVERFLOW image gets d_n_matches = XF_N_OVERFLOW.  Implementations 1-3, XF_E_UNSUPPORTED otherwise;
+ * n_images * n_pad < 2^31; n_pairs <= 65535. */
+XF_API size_t xfeat_mnn_pairs_workspace_bytes(int n_pairs, int n_max);
+XF_API int xfeat_mnn_match_pairs(const void* d_fs, const int32_t* d_n, int n_images, int n_max, int n_pad,
+                          const int32_t* d_pairs, int n_pairs, int scale_log2, float min_cossim,
+                          int64_t* d_idx0, int64_t* d_idx1, int32_t* d_n_matches, void* d_ws, size_t ws_bytes, void* stream);
+/* out0[p][m] = kpts[i][idx0[p][m]], out1[p][m] = kpts[j][idx1[p][m]] for m < n_matches[p]; kpts (n_images, n_max, 2). */
+XF_API int xfeat_gather_matches_pairs(const float* d_kpts, int n_max, const int32_t* d_pairs, const int64_t* d_idx0,
+                               const int64_t* d_idx1, const int32_t* d_n_matches, int n_pairs,
+                               float* d_out0, float* d_out1, void* stream);
+
 XF_API size_t xfeat_refine_workspace_bytes(int batch, int n_max);
 /* replaces: XFeat.refine_matches + fine_matcher + subpix_softmax2d (xfeat.py:292-325, model.py:97-111), for all
  * pairs of the batch at once.  Inputs: un-normalised coarse descriptors d_desc0 (batch,n_max,64) / d_desc1 (batch,n1_max,64),
