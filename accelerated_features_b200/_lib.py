@@ -44,8 +44,12 @@ SIGNATURES = {
     "xfeat_mnn_pairs_workspace_bytes": (c_sz, [c_i, c_i]),
     "xfeat_mnn_match_pairs": (c_i, [c_p, c_p, c_i, c_i, c_i, c_p, c_i, c_i, c_f, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_gather_matches_pairs": (c_i, [c_p, c_i, c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p]),
+    "xfeat_mnn_pairs_f32_workspace_bytes": (c_sz, [c_i, c_i]),
+    "xfeat_mnn_match_pairs_f32": (c_i, [c_p, c_p, c_i, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_refine_workspace_bytes": (c_sz, [c_i, c_i]),
     "xfeat_refine": (c_i, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_i, c_f, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_refine_pairs_workspace_bytes": (c_sz, [c_i, c_i]),
+    "xfeat_refine_pairs": (c_i, [c_p, c_p, c_p, c_p, c_i, c_p, c_p, c_p, c_p, c_i, c_f, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_kpts_heatmap": (c_i, [c_p, c_i, c_i, c_i, c_f, c_p, c_p]),
     "xfeat_nms_workspace_bytes": (c_sz, [c_i, c_i, c_i]),
     "xfeat_nms_count": (c_i, [c_p, c_i, c_i, c_i, c_i, c_f, c_p, c_p, c_sz, c_p]),

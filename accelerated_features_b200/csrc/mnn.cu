@@ -255,6 +255,10 @@ int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const _
 int launch_mnn_fast(const float* f1, const int* n1, int n1_max, int64_t stride1, const float* f2, const int* n2, int n2_max,
                     int64_t stride2, int batch, void* d_ws, size_t ws_bytes, unsigned long long** best12,
                     unsigned long long** best21, float** inv_s2, cudaStream_t st, float abs_bound, int sm_count);
+size_t mnn_tc_pairs_workspace_bytes(int n_pairs, int n_max);
+int launch_mnn_tc_pairs_f32(const float* f, const int* n, int n_max, const int2* pairs, int n_pairs, void* d_ws, size_t ws_bytes,
+                            unsigned long long** best12, unsigned long long** best21, float** inv_s2, const int** cnt1,
+                            const int** cnt2, cudaStream_t st, int variant);
 
 }  // namespace xf
 
@@ -387,6 +391,34 @@ extern "C" int xfeat_mnn_match_pairs(const void* d_fs, const int32_t* d_n, int n
   if (rc) return rc;
   xf::mnn_finalize_kernel<true><<<n_pairs, 1024, 0, st>>>(b12, b21, d_n, d_n, n_max, n_max, min_cossim, inv_s2, (long long*)d_idx0,
                                                     (long long*)d_idx1, d_n_matches, nullptr, 0, nullptr, 0, pairs);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" size_t xfeat_mnn_pairs_f32_workspace_bytes(int n_pairs, int n_max) {
+  return xf::mnn_tc_pairs_workspace_bytes(n_pairs, n_max);
+}
+
+extern "C" int xfeat_mnn_match_pairs_f32(const float* d_f, const int32_t* d_n, int n_images, int n_max, const int32_t* d_pairs,
+                                         int n_pairs, int64_t* d_idx0, int64_t* d_idx1, int32_t* d_n_matches, void* d_ws,
+                                         size_t ws_bytes, void* stream) {
+  XF_REQUIRE(d_f && d_n && d_pairs && d_idx0 && d_idx1 && d_n_matches && d_ws, "mnn_match_pairs_f32: null pointer");
+  XF_REQUIRE(n_images > 0 && n_pairs > 0 && n_pairs <= 65535 && n_max > 0, "mnn_match_pairs_f32: bad sizes");
+  XF_REQUIRE(((uintptr_t)d_f % 16) == 0, "mnn_match_pairs_f32: descriptors must be 16-byte aligned");
+  XF_REQUIRE(((uintptr_t)d_pairs % 8) == 0, "mnn_match_pairs_f32: the pair table must be 8-byte aligned");
+  if (xf::g_mnn_impl < 1 || xf::g_mnn_impl > 3) {
+    xf::set_error("mnn_match_pairs_f32: implementation %d does not take pre-split operands (1, 2 and 3 do)", xf::g_mnn_impl);
+    return XF_E_UNSUPPORTED;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long *b12 = nullptr, *b21 = nullptr;
+  float* inv_s2 = nullptr;
+  const int *n1 = nullptr, *n2 = nullptr;
+  int rc = xf::launch_mnn_tc_pairs_f32(d_f, d_n, n_max, reinterpret_cast<const int2*>(d_pairs), n_pairs, d_ws, ws_bytes, &b12,
+                                       &b21, &inv_s2, &n1, &n2, st, xf::g_mnn_impl - 1);
+  if (rc) return rc;
+  xf::mnn_finalize_kernel<<<n_pairs, 1024, 0, st>>>(b12, b21, n1, n2, n_max, n_max, -1.f, inv_s2, (long long*)d_idx0,
+                                                    (long long*)d_idx1, d_n_matches);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -32,11 +32,17 @@ PFN_encodeTiled get_encode_tiled() {
 constexpr int TC_ROWS = 256, TC_BN = 128, TC_KP = 128, TC_BOX_BYTES = 128 * 128;  // operand row [hi(64) | lo(64)]; box = 128 rows x 128 B
 constexpr size_t TC_SMEM = 1024 + 8 * (size_t)TC_BOX_BYTES + 256;
 
+// max |x| over the first n rows of each set into *out.  kPairs: one word per pair instead -- out[p] = max |x| over the first n
+// rows of both images of pairs[p] = (i, j) (blockIdx.z = side) of one table of images at `stride` floats each, exactly the
+// maximum the single-pair launch measures over its two sets.  A template flag, so that the per-set build keeps its code.
+template <bool kPairs = false>
 __global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ f, const int* __restrict__ np, int n_max,
-                                                     int64_t stride, unsigned* __restrict__ out) {
+                                                     int64_t stride, unsigned* __restrict__ out,
+                                                     const int2* __restrict__ pairs = nullptr) {
   const int pair = blockIdx.y;
-  const int n = np ? min(np[pair], n_max) : n_max;
-  const float4* p = reinterpret_cast<const float4*>(f + (int64_t)pair * stride);
+  const int set = kPairs ? (blockIdx.z ? __ldg(pairs + pair).y : __ldg(pairs + pair).x) : pair;
+  const int n = np ? min(np[set], n_max) : n_max;
+  const float4* p = reinterpret_cast<const float4*>(f + (int64_t)set * stride);
   float m = 0.f;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n * 16; i += gridDim.x * blockDim.x) {
     const float4 v = __ldg(p + i);
@@ -44,32 +50,40 @@ __global__ void __launch_bounds__(256) absmax_kernel(const float* __restrict__ f
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));
+  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out + (kPairs ? pair : 0), __float_as_uint(m));
 }
 
 // One warp per row: writes the 128-half split row [hi(64) | lo(64)]; zero rows past n.
+// kPairs: pair p = pairs[p] = (i, j) of one table of images at `stride` floats each; side s = blockIdx.z splits the rows of
+// image (s ? j : i) at the exponent of the pair's own maximum absmax[p] (absmax_kernel<true>) into block s * gridDim.y + p of
+// `out` (side 0: the pairs' A rows, side 1: their B rows), and writes that image's count to cnt[s * gridDim.y + p].
+template <bool kPairs = false>
 __global__ void __launch_bounds__(256) split_kernel(const float* __restrict__ f, const int* __restrict__ np, int n_max,
                                                     int n_pad, int64_t stride, const unsigned* __restrict__ absmax,
-                                                    float abs_bound, __half* __restrict__ out, float* __restrict__ inv_s2) {
+                                                    float abs_bound, __half* __restrict__ out, float* __restrict__ inv_s2,
+                                                    const int2* __restrict__ pairs = nullptr, int* __restrict__ cnt = nullptr) {
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const int pair = blockIdx.y;
   if (wid >= n_pad) return;
-  const int n = np ? min(np[pair], n_max) : n_max;
-  const float mx = abs_bound > 0.f ? abs_bound : __uint_as_float(*absmax);   // caller's bound or the measured maximum
+  const int set = kPairs ? (blockIdx.z ? __ldg(pairs + pair).y : __ldg(pairs + pair).x) : pair;
+  const int blk = kPairs ? (int)(blockIdx.z * gridDim.y) + pair : pair;
+  const int n = np ? min(np[set], n_max) : n_max;
+  const float mx = abs_bound > 0.f ? abs_bound : __uint_as_float(absmax[kPairs ? pair : 0]);   // caller's bound or the measured maximum
   int e = 0;
   if (mx > 0.f) frexpf(mx, &e);                 // mx = m * 2^e, m in [0.5, 1)  ->  mx < 2^e
   const float s = (mx > 0.f) ? ldexpf(1.f, 14 - e) : 1.f;   // mx * s in [2^13, 2^14)
   if (wid == 0 && lane == 0 && pair == 0 && inv_s2) *inv_s2 = (mx > 0.f) ? ldexpf(1.f, 2 * (e - 14)) : 1.f;
+  if (kPairs && wid == 0 && lane == 0) cnt[blk] = np[set];
   __half2 hi = __floats2half2_rn(0.f, 0.f), lo = hi;
   if (wid < n) {
-    const float2 v = __ldg(reinterpret_cast<const float2*>(f + (int64_t)pair * stride + wid * 64) + lane);
+    const float2 v = __ldg(reinterpret_cast<const float2*>(f + (int64_t)set * stride + wid * 64) + lane);
     const float x0 = v.x * s, x1 = v.y * s;      // exact (power of two)
     hi = __floats2half2_rn(x0, x1);
     const float2 hf = __half22float2(hi);
     lo = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
   }
-  __half2* o = reinterpret_cast<__half2*>(out + ((int64_t)pair * n_pad + wid) * TC_KP);
+  __half2* o = reinterpret_cast<__half2*>(out + ((int64_t)blk * n_pad + wid) * TC_KP);
   o[lane] = hi;
   o[32 + lane] = lo;
 }
@@ -764,6 +778,60 @@ int launch_mnn_tc_presplit(const __half* f1s, const int* n1, int n1_max, const _
   if ((rc = make_map(&maps.m1, f1s, (uint64_t)table_rows))) return rc;
   if ((rc = make_map(&maps.m2, f2s, (uint64_t)table_rows))) return rc;
   return launch_mnn_tc_main(maps, n1, n1_max, n2, n2_max, n_pad, batch, b12, b21, st, variant, pairs);
+}
+
+// Pair lists over one fp32 image table (xfeat_mnn_match_pairs_f32): f (n_images, n_max, 64), n (n_images) counts.  Pair p is
+// split at the exponent of its own maximum -- max |x| over its two images, the one launch_mnn_tc measures for that pair alone --
+// into per-pair operand blocks (A rows at p * n_pad of one array, B rows at p * n_pad of the other, with per-pair counts) that
+// the presplit kernels match as they stand.  One exponent per image or per table would change the lo terms (and the tiny hi
+// terms) that round into fp16 subnormals, hence S in its last bits, hence near-tie arg-maxes.
+struct MnnPairsWs {
+  __half* ops;
+  unsigned* absmax;
+  int* cnt;
+};
+static void carve_mnn_pairs(Bump& bump, int n_pairs, int n_max, MnnPairsWs& ws) {
+  ws.ops = bump.take<__half>((size_t)2 * n_pairs * tc_pad(n_max) * TC_KP);
+  ws.absmax = bump.take<unsigned>(n_pairs);
+  ws.cnt = bump.take<int>((size_t)2 * n_pairs);
+  bump.take<unsigned long long>((size_t)n_pairs * n_max);   // the presplit launch's best12 / best21 / scale, carved by it
+  bump.take<unsigned long long>((size_t)n_pairs * n_max);
+  bump.take<float>(1);
+}
+
+size_t mnn_tc_pairs_workspace_bytes(int n_pairs, int n_max) {
+  Bump bump(nullptr, 0);
+  MnnPairsWs ws;
+  carve_mnn_pairs(bump, n_pairs, n_max, ws);
+  return bump.used();
+}
+
+int launch_mnn_tc_pairs_f32(const float* f, const int* n, int n_max, const int2* pairs, int n_pairs, void* d_ws, size_t ws_bytes,
+                            unsigned long long** best12, unsigned long long** best21, float** inv_s2, const int** cnt1,
+                            const int** cnt2, cudaStream_t st, int variant) {
+  const int n_pad = tc_pad(n_max);
+  XF_REQUIRE((int64_t)n_pairs * n_pad < (1ll << 31), "mnn_match_pairs_f32: n_pairs * n too large");
+  Bump bump(d_ws, ws_bytes);
+  MnnPairsWs ws;
+  carve_mnn_pairs(bump, n_pairs, n_max, ws);
+  if (!bump.ok) {
+    set_error("mnn_match_pairs_f32: workspace too small (%zu < %zu)", ws_bytes, bump.used());
+    return XF_E_WORKSPACE;
+  }
+  const int64_t stride = (int64_t)n_max * 64;
+  XF_CUDA(cudaMemsetAsync(ws.absmax, 0, sizeof(unsigned) * (size_t)n_pairs, st));
+  absmax_kernel<true><<<dim3(8, n_pairs, 2), 256, 0, st>>>(f, n, n_max, stride, ws.absmax, pairs);
+  XF_LAUNCH_CHECK();
+  split_kernel<true><<<dim3(cdiv(n_pad * 32, 256), n_pairs, 2), 256, 0, st>>>(f, n, n_max, n_pad, stride, ws.absmax, 0.f, ws.ops,
+                                                                              nullptr, pairs, ws.cnt);
+  XF_LAUNCH_CHECK();
+  *cnt1 = ws.cnt;
+  *cnt2 = ws.cnt + n_pairs;
+  const size_t head = (size_t)((char*)(ws.cnt + 2 * (size_t)n_pairs) - (char*)d_ws);
+  const size_t off = (head + 255) / 256 * 256;   // the rest of the workspace: what carve_mnn_pairs reserved for this launch
+  // scale_log2 only feeds the min_cossim test, which this path does not run
+  return launch_mnn_tc_presplit(ws.ops, ws.cnt, n_max, ws.ops + (size_t)n_pairs * n_pad * TC_KP, ws.cnt + n_pairs, n_max, n_pad,
+                                n_pairs, 0, (char*)d_ws + off, ws_bytes - off, best12, best21, inv_s2, st, variant, nullptr, 0);
 }
 
 int launch_absmax(const float* f, const int* np, int n_max, int64_t stride, int batch, unsigned* out, cudaStream_t st) {

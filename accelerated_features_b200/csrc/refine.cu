@@ -34,12 +34,16 @@ __global__ void __launch_bounds__(1024) scan_counts_kernel(const int* __restrict
 }
 
 // warp per (pair, m): X[row] = [desc0[pair][idx0[m]], desc1[pair][idx1[m]]]
+// kPairs: pair p = pairs[p] = (i, j) reads desc0[i] and desc1[j] of one table (both at stride n_max = n1_max) -- the image slots
+// of xfeat_refine_pairs.  A template flag, so that the per-pair build keeps its code.
+template <bool kPairs = false>
 __global__ void __launch_bounds__(256) refine_gather_kernel(const float* __restrict__ d0, const float* __restrict__ d1,
                                                             const long long* __restrict__ idx0,
                                                             const long long* __restrict__ idx1,
                                                             const int* __restrict__ n_matches,
                                                             const int* __restrict__ offsets, int batch, int n_max,
-                                                            int n1_max, float* __restrict__ X, __half* __restrict__ Xs) {
+                                                            int n1_max, float* __restrict__ X, __half* __restrict__ Xs,
+                                                            const int2* __restrict__ pairs = nullptr) {
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (wid >= (int64_t)batch * n_max) return;
@@ -47,8 +51,9 @@ __global__ void __launch_bounds__(256) refine_gather_kernel(const float* __restr
   if (m >= min(n_matches[pair], n_max)) return;
   const int64_t row = offsets[pair] + m;
   const long long a = idx0[wid], b = idx1[wid];
-  const float2 u = __ldg(reinterpret_cast<const float2*>(d0 + ((int64_t)pair * n_max + a) * 64) + lane);
-  const float2 v = __ldg(reinterpret_cast<const float2*>(d1 + ((int64_t)pair * n1_max + b) * 64) + lane);
+  const int2 ij = kPairs ? __ldg(pairs + pair) : make_int2(pair, pair);
+  const float2 u = __ldg(reinterpret_cast<const float2*>(d0 + ((int64_t)ij.x * n_max + a) * 64) + lane);
+  const float2 v = __ldg(reinterpret_cast<const float2*>(d1 + ((int64_t)ij.y * n1_max + b) * 64) + lane);
   if (Xs) {   // tensor-core MLP: split fp16 row [hi(128) | lo(128)] (mlp_tc.cu)
     const __half2 uh = __floats2half2_rn(u.x, u.y), vh = __floats2half2_rn(v.x, v.y);
     const float2 uf = __half22float2(uh), vf = __half22float2(vh);
@@ -64,6 +69,8 @@ __global__ void __launch_bounds__(256) refine_gather_kernel(const float* __restr
 }
 
 // warp per (pair, m): softmax(3*o) statistics -> tmp[wid] = (x0', y0', x1, y1, keep)
+// kPairs: k0 / sc0 of image i and k1 of image j of pairs[p] = (i, j), as in refine_gather_kernel
+template <bool kPairs = false>
 __global__ void __launch_bounds__(256) refine_finish_kernel(const float* __restrict__ logits,
                                                             const float* __restrict__ k0, const float* __restrict__ k1,
                                                             const float* __restrict__ sc0,
@@ -72,7 +79,7 @@ __global__ void __launch_bounds__(256) refine_finish_kernel(const float* __restr
                                                             const int* __restrict__ n_matches,
                                                             const int* __restrict__ offsets, int batch, int n_max,
                                                             int n1_max, float fine_conf, float* __restrict__ tmp,
-                                                            int* __restrict__ keep) {
+                                                            int* __restrict__ keep, const int2* __restrict__ pairs = nullptr) {
   const int64_t wid = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (wid >= (int64_t)batch * n_max) return;
@@ -98,9 +105,10 @@ __global__ void __launch_bounds__(256) refine_finish_kernel(const float* __restr
   if (lane == 0) {
     const float conf = 1.0f / s;  // max of the softmax = exp(0)/sum
     const long long a = idx0[wid], b = idx1[wid];
-    const float scale = __ldg(sc0 + (int64_t)pair * n_max + a);
-    const float2 p0 = __ldg(reinterpret_cast<const float2*>(k0) + (int64_t)pair * n_max + a);
-    const float2 p1 = __ldg(reinterpret_cast<const float2*>(k1) + (int64_t)pair * n1_max + b);
+    const int2 ij = kPairs ? __ldg(pairs + pair) : make_int2(pair, pair);
+    const float scale = __ldg(sc0 + (int64_t)ij.x * n_max + a);
+    const float2 p0 = __ldg(reinterpret_cast<const float2*>(k0) + (int64_t)ij.x * n_max + a);
+    const float2 p1 = __ldg(reinterpret_cast<const float2*>(k1) + (int64_t)ij.y * n1_max + b);
     float* t = tmp + wid * 4;
     t[0] = p0.x + (sx / s) * scale;  // mkpts_0 += offsets * sc0 (xfeat.py:319)
     t[1] = p0.y + (sy / s) * scale;
@@ -172,16 +180,12 @@ extern "C" size_t xfeat_refine_workspace_bytes(int batch, int n_max) {
   return bump.used();
 }
 
-extern "C" int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d_desc1, const float* d_kpts0,
-                            const float* d_kpts1, const float* d_scales0, const int64_t* d_idx0, const int64_t* d_idx1,
-                            const int32_t* d_n_matches, int batch, int n_max, int n1_max, float fine_conf, float* d_matches,
-                            int32_t* d_n_refined, void* d_ws, size_t ws_bytes, void* stream) {
-  XF_REQUIRE(ctx && d_desc0 && d_desc1 && d_kpts0 && d_kpts1 && d_scales0 && d_idx0 && d_idx1 && d_n_matches &&
-                 d_matches && d_n_refined && d_ws,
-             "refine: null pointer");
-  XF_REQUIRE(batch > 0 && batch <= 65535 && n_max > 0 && n1_max > 0 && (int64_t)batch * n_max < (1ll << 31), "refine: bad sizes");
+// xfeat_refine and xfeat_refine_pairs: pairs == NULL -> pair p reads slot p of desc0 / desc1 / kpts0 / kpts1 / scales0.
+static int refine_impl(xfeat_ctx* ctx, const float* d_desc0, const float* d_desc1, const float* d_kpts0, const float* d_kpts1,
+                       const float* d_scales0, const int64_t* d_idx0, const int64_t* d_idx1, const int32_t* d_n_matches, int batch,
+                       int n_max, int n1_max, float fine_conf, float* d_matches, int32_t* d_n_refined, void* d_ws,
+                       size_t ws_bytes, cudaStream_t st, const int2* pairs) {
   XF_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
   xf::Bump bump(d_ws, ws_bytes);
   xf::RefineWs ws;
   xf::carve_refine(bump, batch, n_max, ws);
@@ -194,9 +198,14 @@ extern "C" int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d
   const bool tc = xf::g_conv_impl != 0;   // xfeat_set_conv_impl(0): everything on the fp32 CUDA-core kernels (A/B reference)
   xf::scan_counts_kernel<<<1, 1024, 0, st>>>(d_n_matches, batch, n_max, ws.offsets);
   XF_LAUNCH_CHECK();
-  xf::refine_gather_kernel<<<wblocks, 256, 0, st>>>(d_desc0, d_desc1, (const long long*)d_idx0, (const long long*)d_idx1,
-                                                    d_n_matches, ws.offsets, batch, n_max, n1_max, ws.X,
-                                                    tc ? (__half*)ws.X : nullptr);
+  if (pairs)
+    xf::refine_gather_kernel<true><<<wblocks, 256, 0, st>>>(d_desc0, d_desc1, (const long long*)d_idx0, (const long long*)d_idx1,
+                                                            d_n_matches, ws.offsets, batch, n_max, n1_max, ws.X,
+                                                            tc ? (__half*)ws.X : nullptr, pairs);
+  else
+    xf::refine_gather_kernel<<<wblocks, 256, 0, st>>>(d_desc0, d_desc1, (const long long*)d_idx0, (const long long*)d_idx1,
+                                                      d_n_matches, ws.offsets, batch, n_max, n1_max, ws.X,
+                                                      tc ? (__half*)ws.X : nullptr);
   XF_LAUNCH_CHECK();
   const int* n_live = ws.offsets + batch;
   int rc;
@@ -206,11 +215,42 @@ extern "C" int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d
   } else if ((rc = xf::launch_fine_mlp(ctx, ws.X, (int)cap, n_live, ws.actA, ws.actB, ws.logits, st))) {
     return rc;
   }
-  xf::refine_finish_kernel<<<wblocks, 256, 0, st>>>(ws.logits, d_kpts0, d_kpts1, d_scales0, (const long long*)d_idx0,
-                                                    (const long long*)d_idx1, d_n_matches, ws.offsets, batch, n_max, n1_max,
-                                                    fine_conf, ws.tmp, ws.keep);
+  if (pairs)
+    xf::refine_finish_kernel<true><<<wblocks, 256, 0, st>>>(ws.logits, d_kpts0, d_kpts1, d_scales0, (const long long*)d_idx0,
+                                                            (const long long*)d_idx1, d_n_matches, ws.offsets, batch, n_max,
+                                                            n1_max, fine_conf, ws.tmp, ws.keep, pairs);
+  else
+    xf::refine_finish_kernel<<<wblocks, 256, 0, st>>>(ws.logits, d_kpts0, d_kpts1, d_scales0, (const long long*)d_idx0,
+                                                      (const long long*)d_idx1, d_n_matches, ws.offsets, batch, n_max, n1_max,
+                                                      fine_conf, ws.tmp, ws.keep);
   XF_LAUNCH_CHECK();
   xf::refine_compact_kernel<<<batch, 1024, 0, st>>>(ws.tmp, ws.keep, d_n_matches, n_max, d_matches, d_n_refined);
   XF_LAUNCH_CHECK();
   return XF_OK;
+}
+
+extern "C" int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d_desc1, const float* d_kpts0,
+                            const float* d_kpts1, const float* d_scales0, const int64_t* d_idx0, const int64_t* d_idx1,
+                            const int32_t* d_n_matches, int batch, int n_max, int n1_max, float fine_conf, float* d_matches,
+                            int32_t* d_n_refined, void* d_ws, size_t ws_bytes, void* stream) {
+  XF_REQUIRE(ctx && d_desc0 && d_desc1 && d_kpts0 && d_kpts1 && d_scales0 && d_idx0 && d_idx1 && d_n_matches &&
+                 d_matches && d_n_refined && d_ws,
+             "refine: null pointer");
+  XF_REQUIRE(batch > 0 && batch <= 65535 && n_max > 0 && n1_max > 0 && (int64_t)batch * n_max < (1ll << 31), "refine: bad sizes");
+  return refine_impl(ctx, d_desc0, d_desc1, d_kpts0, d_kpts1, d_scales0, d_idx0, d_idx1, d_n_matches, batch, n_max, n1_max,
+                     fine_conf, d_matches, d_n_refined, d_ws, ws_bytes, (cudaStream_t)stream, nullptr);
+}
+
+extern "C" size_t xfeat_refine_pairs_workspace_bytes(int n_pairs, int n_max) { return xfeat_refine_workspace_bytes(n_pairs, n_max); }
+
+extern "C" int xfeat_refine_pairs(xfeat_ctx* ctx, const float* d_desc, const float* d_kpts, const float* d_scales, int n_max,
+                                  const int32_t* d_pairs, const int64_t* d_idx0, const int64_t* d_idx1,
+                                  const int32_t* d_n_matches, int n_pairs, float fine_conf, float* d_matches,
+                                  int32_t* d_n_refined, void* d_ws, size_t ws_bytes, void* stream) {
+  XF_REQUIRE(ctx && d_desc && d_kpts && d_scales && d_pairs && d_idx0 && d_idx1 && d_n_matches && d_matches && d_n_refined && d_ws,
+             "refine_pairs: null pointer");
+  XF_REQUIRE(n_pairs > 0 && n_pairs <= 65535 && n_max > 0 && (int64_t)n_pairs * n_max < (1ll << 31), "refine_pairs: bad sizes");
+  XF_REQUIRE(((uintptr_t)d_pairs % 8) == 0, "refine_pairs: the pair table must be 8-byte aligned");
+  return refine_impl(ctx, d_desc, d_desc, d_kpts, d_kpts, d_scales, d_idx0, d_idx1, d_n_matches, n_pairs, n_max, n_max, fine_conf,
+                     d_matches, d_n_refined, d_ws, ws_bytes, (cudaStream_t)stream, reinterpret_cast<const int2*>(d_pairs));
 }

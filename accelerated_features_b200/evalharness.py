@@ -2,7 +2,7 @@
 
 `modules/eval/megadepth1500.py:200-237` (run_pose_benchmark) and `modules/eval/scannet1500.py:207-230` call
 `matcher_fn(bgr0, bgr1)` one pair at a time, 1500 times.  Here the same protocol runs the matcher over the whole list of pairs
-(sparse: XFeat.match_xfeat_pairs, each distinct image extracted once; semi-dense: batches grouped by image shape) and returns
+(sparse: XFeat.match_xfeat_pairs, semi-dense: XFeat.match_xfeat_star_pairs; each distinct image extracted once) and returns
 the matches in the callers' order, so the pose / AUC stage downstream is unchanged.  The metric functions are
 restated from the reference (citations on each) because its module imports poselib at import time, which is not installed
 here; the pose estimator is pluggable (default: OpenCV's 5-point RANSAC as a stand-in for poselib)."""
@@ -16,12 +16,14 @@ import numpy as np
 def batched_matcher(xf, mode: str = "sparse", top_k=None, batch_size: int = 64) -> Callable[[Sequence[Tuple[np.ndarray, np.ndarray]]], List[Tuple[np.ndarray, np.ndarray]]]:
     """-> match_pairs(pairs): pairs = [(img0, img1)] numpy (H,W,3) uint8 images (any mix of shapes) -> [(mkpts0, mkpts1)] in the
     same order; what [matcher_fn(a, b) for a, b in pairs] returns with matcher_fn = xfeat.match_xfeat / match_xfeat_star.
-    sparse: one match_xfeat_pairs call over the list, an image object that appears in several pairs is extracted once (images
-    are told apart by identity); star: chunks of `batch_size` pairs of one (shape0, shape1) through match_xfeat_star."""
+    One call over the whole list -- sparse: match_xfeat_pairs, star: match_xfeat_star_pairs -- in which an image object that
+    appears in several pairs is extracted once (images are told apart by identity).  `batch_size` is not used any more (both
+    modes size their launches themselves); it stays for the callers that pass it."""
     if mode not in ("sparse", "star"):
         raise ValueError("mode must be 'sparse' or 'star'")
+    match_list = xf.match_xfeat_pairs if mode == "sparse" else xf.match_xfeat_star_pairs
 
-    def match_sparse(pairs):
+    def match_pairs(pairs):
         images: List[np.ndarray] = []
         slot: Dict[int, int] = {}
         idx = []
@@ -31,27 +33,7 @@ def batched_matcher(xf, mode: str = "sparse", top_k=None, batch_size: int = 64) 
                     slot[id(im)] = len(images)
                     images.append(im)
             idx.append([slot[id(pair[0])], slot[id(pair[1])]])
-        return xf.match_xfeat_pairs(images, np.asarray(idx, np.int64).reshape(-1, 2), top_k=top_k)
-
-    def match_pairs(pairs):
-        pairs = list(pairs)
-        if mode == "sparse":
-            return match_sparse(pairs)
-        out: List = [None] * len(pairs)
-        groups: Dict[tuple, List[int]] = {}
-        for i, (a, b) in enumerate(pairs):
-            groups.setdefault((a.shape, a.dtype.str, b.shape, b.dtype.str), []).append(i)
-        for idxs in groups.values():
-            for ch in (idxs[o:o + batch_size] for o in range(0, len(idxs), batch_size)):
-                a = np.stack([pairs[i][0] for i in ch]); b = np.stack([pairs[i][1] for i in ch])
-                res = xf.match_xfeat_star(a, b, top_k=top_k)
-                if len(ch) == 1:
-                    out[ch[0]] = res                                  # B == 1: two numpy arrays (xfeat.py:217)
-                else:
-                    for i, m in zip(ch, res):
-                        m = m.cpu().numpy()
-                        out[i] = (m[:, :2], m[:, 2:])
-        return out
+        return match_list(images, np.asarray(idx, np.int64).reshape(-1, 2), top_k=top_k)
 
     return match_pairs
 

@@ -8,7 +8,8 @@ There is no CPU / eager fallback: without a CUDA device and the built library th
 Beyond the reference surface: `match_xfeat_batch` (batched match_xfeat) and `match_xfeat_stream` (pinned, double-buffered
 host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match_lighterglue_batch` and
 `match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu), `match_xfeat_pairs` and
-`match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once).
+`match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once), and
+`match_xfeat_star_pairs` (the same for semi-dense matching: XFeat* over a list of pairs, each image extracted once per scale).
 """
 from __future__ import annotations
 
@@ -36,6 +37,9 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
 # ----------------------------------------------------------------------------------------------------------------------
 PAIRS_EXTRACT_CHUNK = 64      # images per extraction launch sequence
 PAIRS_MATCH_CHUNK = 4096      # pairs per matcher launch (and per host synchronisation)
+# device bytes per match_xfeat_star_pairs matcher chunk (split operands, matcher and refine workspaces, outputs): about 39 pairs
+# at 10 000 rows per image, 96 at 4096; the image table and the extraction come on top
+STAR_PAIRS_MATCH_BYTES = 2 << 30
 
 
 def pair_image_key(x) -> tuple:
@@ -70,6 +74,58 @@ def check_pairs(pairs, n_images: int) -> np.ndarray:
         bad = np.nonzero((a < 0).any(1) | (a >= n_images).any(1))[0]
         raise ValueError(f"pairs {bad[:8].tolist()} index outside the {n_images} images")
     return a.astype(np.int64)
+
+
+def _dense_cells(h: int, w: int) -> int:
+    """1/8-resolution cells of an h x w image after preprocess_tensor's crop to multiples of 32 (xfeat.py:229-231)."""
+    return ((h // 32) * 32 // 8) * ((w // 32) * 32 // 8)
+
+
+def _dense_cap(top_k: int) -> int:
+    return 100_000_000 if top_k < 1 else top_k           # extractDense: `if top_k < 1: top_k = 100_000_000` (xfeat.py:357-358)
+
+
+def dense_counts(H: int, W: int, top_k: int, s1: float = 0.6, s2: float = 1.3) -> Tuple[int, int]:
+    """Rows (k1, k2) that extract_dualscale gives an H x W image at its two scales (xfeat.py:379-394): the first scale keeps
+    int(top_k * 0.2) cells, the second int(top_k * 0.8), each capped by the cells of the rescaled image, and a cap below 1 means
+    unlimited (so top_k = 4 leaves the first scale unlimited).  A scale whose image is under 32 pixels gives 0 rows."""
+    t1, t2 = _dense_cap(int(top_k * 0.20)), _dense_cap(int(top_k * 0.80))      # xfeat.py:385-386
+    k1 = min(_dense_cells(int(math.floor(H * s1)), int(math.floor(W * s1))), t1)
+    k2 = min(_dense_cells(int(math.floor(H * s2)), int(math.floor(W * s2))), t2)
+    return k1, k2
+
+
+def star_pair_rows(keys, plan: "PairPlan", top_k: int) -> np.ndarray:
+    """(n_slots,) int32: dense rows k1 + k2 of each planned image of match_xfeat_star_pairs.  Raises, naming the image, for an
+    image match_xfeat_star would refuse (under 32 pixels after the 0.6 rescale)."""
+    rows = np.zeros(plan.n_slots, np.int32)
+    for i in np.nonzero(plan.slot >= 0)[0].tolist():
+        H, W = keys[i][1], keys[i][2]
+        k1, k2 = dense_counts(H, W, top_k)
+        if k1 == 0 or k2 == 0:
+            raise RuntimeError(f"match_xfeat_star_pairs: image {i} ({H}x{W}): image smaller than 32 pixels after the 0.6 rescale")
+        rows[plan.slot[i]] = k1 + k2
+    return rows
+
+
+# carve_refine (csrc/refine.cu) per coarse-row slot: X (128), two MLP activations (512 each), logits (64), tmp (4), keep (1)
+_REFINE_ROW_BYTES = 4 * (128 + 512 + 512 + 64 + 4 + 1)
+
+
+def star_pair_bytes(k_max: int) -> int:
+    """Device bytes one pair of a match_xfeat_star_pairs chunk needs at k_max rows per image: [hi | lo] operand rows of both
+    sides (512 B per padded row), best12 / best21, idx0 / idx1, the refine workspace and the refined matches, plus 2 KB for the
+    workspaces' 256-byte alignment."""
+    n_pad = (k_max + 511) // 512 * 512
+    return 2 * n_pad * 256 + k_max * (2 * 8 + 2 * 8 + _REFINE_ROW_BYTES + 16) + 2048
+
+
+def star_match_chunks(n_pairs: int, k_max: int, budget: Optional[int] = None) -> List[Tuple[int, int]]:
+    """[start, stop) ranges of the matched pairs: as many pairs per chunk as fit in `budget` bytes (STAR_PAIRS_MATCH_BYTES), at
+    least one, at most 65535 (the kernels' grid limit)."""
+    budget = STAR_PAIRS_MATCH_BYTES if budget is None else budget
+    step = max(1, min(65535, budget // star_pair_bytes(k_max)))
+    return [(o, min(o + step, n_pairs)) for o in range(0, n_pairs, step)]
 
 
 class PairPlan:
@@ -693,14 +749,23 @@ class XFeat(torch.nn.Module):
 
     def _extract_table(self, images, plan: PairPlan, top_k: int, want_split: bool, want_desc: bool) -> Dict[str, torch.Tensor]:
         """Sparse extraction of every planned image into one table (row = slot): keypoints (n, top_k, 2), n_valid (n) and the
-        descriptors (n, top_k, 64) and / or operand rows (n, split_rows, 128).  The chunks go through match_xfeat_stream's copy
-        pipeline: chunk c+1 is uploaded on the copy stream while chunk c is extracted.  No host sync."""
+        descriptors (n, top_k, 64) and / or operand rows (n, split_rows, 128).  No host sync."""
         n = plan.n_slots
         tab = {"keypoints": self._empty((n, top_k, 2)), "n_valid": self._empty((n,), torch.int32)}
         if want_desc:
             tab["descriptors"] = self._empty((n, top_k, 64))
         if want_split:
             tab["desc_split"] = self._empty((n, self._split_rows(top_k), 128), torch.float16)
+
+        def step(cur, out):
+            self._detect_sparse_device([x for x, _ in cur], top_k, self.detection_threshold, [f for _, f in cur],
+                                       want_split=want_split, want_desc=want_desc, out=out)
+        return self._fill_table(images, plan, tab, step)
+
+    def _fill_table(self, images, plan: PairPlan, tab: Dict[str, torch.Tensor], step) -> Dict[str, torch.Tensor]:
+        """Run `step(batches, out)` over the plan's chunks: `batches` is the chunk's images on the device, [((1,C,H,W) tensor,
+        div255)] of one bucket, and `out` = {name: table[s0:s1]} the chunk's slots of every table in `tab`.  The chunks go
+        through match_xfeat_stream's copy pipeline: chunk c+1 is uploaded on the copy stream while chunk c is extracted."""
         if self._pipe is None:
             self._pipe = XFeat._Pipe(self.dev)
         pipe = self._pipe
@@ -717,8 +782,7 @@ class XFeat(torch.nn.Module):
             nxt = upload(c + 1, slot ^ 1) if c + 1 < len(plan.chunks) else None     # overlaps the kernels queued below
             main.wait_event(pipe.ready[slot])
             s1 = s0 + len(chunk)
-            self._detect_sparse_device([x for x, _ in cur], top_k, self.detection_threshold, [f for _, f in cur],
-                                       want_split=want_split, want_desc=want_desc, out={k: v[s0:s1] for k, v in tab.items()})
+            step(cur, {k: v[s0:s1] for k, v in tab.items()})
             pipe.freed[slot].record(main)
             cur, s0 = nxt, s1
         return tab
@@ -871,23 +935,21 @@ class XFeat(torch.nn.Module):
         Hi, Wi = x.shape[-2:]
         return self._resize(x, div255, int(math.floor(Hi * s)), int(math.floor(Wi * s)), 1.0 / s, 1.0 / s)
 
-    @staticmethod
-    def _cells_of(h: int, w: int) -> int:
-        return ((h // 32) * 32 // 8) * ((w // 32) * 32 // 8)
-
-    @staticmethod
-    def _unlimited(top_k: int) -> int:
-        return 100_000_000 if top_k < 1 else top_k           # extractDense: `if top_k < 1: top_k = 100_000_000` (xfeat.py:357-358)
-
-    def _dense_device(self, x, top_k: int, multiscale: bool, div255: bool = False, s1: float = 0.6, s2: float = 1.3):
+    def _dense_device(self, x, top_k: int, multiscale: bool, div255: bool = False, s1: float = 0.6, s2: float = 1.3,
+                      out: Optional[Dict[str, torch.Tensor]] = None):
+        """`out` (multiscale): write 'keypoints', 'descriptors' and 'scales' into these (B, K_max, ...) tensors, e.g. slices of
+        an image table with K_max >= k1 + k2 rows per image, instead of fresh (B, k1 + k2, ...) ones; rows past k1 + k2 are not
+        written."""
         x = self._to_bchw(x)
         B, _, Hi, Wi = x.shape
         if multiscale:
-            t1, t2 = self._unlimited(int(top_k * 0.20)), self._unlimited(int(top_k * 0.80))      # xfeat.py:385-386
-            k1 = min(self._cells_of(int(math.floor(Hi * s1)), int(math.floor(Wi * s1))), t1)
-            k2 = min(self._cells_of(int(math.floor(Hi * s2)), int(math.floor(Wi * s2))), t2)
-            K = k1 + k2
-            kpts, desc, scales = self._empty((B, K, 2)), self._empty((B, K, 64)), self._empty((B, K))
+            k1, k2 = dense_counts(Hi, Wi, top_k, s1, s2)
+            if out is None:
+                K = k1 + k2
+                kpts, desc, scales = self._empty((B, K, 2)), self._empty((B, K, 64)), self._empty((B, K))
+            else:
+                kpts, desc, scales = out["keypoints"], out["descriptors"], out["scales"]
+                K = kpts.shape[1]
             for s, k, off in ((s1, k1, 0), (s2, k2, k1)):
                 Hs, Ws = int(math.floor(Hi * s)), int(math.floor(Wi * s))
                 if Hs % 32 == 0 and Ws % 32 == 0:
@@ -898,7 +960,7 @@ class XFeat(torch.nn.Module):
                     self._extract_dense_into(xs, False, k, s, 1 / s, K, off, kpts, desc, scales)
                     del xs
         else:
-            K = min(self._cells_of(Hi, Wi), self._unlimited(top_k))
+            K = min(_dense_cells(Hi, Wi), _dense_cap(top_k))
             kpts, desc, scales = self._empty((B, K, 2)), self._empty((B, K, 64)), self._empty((B, K))
             self._extract_dense_into(x, div255, K, 1.0, 1.0, K, 0, kpts, desc, scales)
         return {"keypoints": kpts, "descriptors": desc, "scales": scales}
@@ -965,6 +1027,91 @@ class XFeat(torch.nn.Module):
         n = n_ref.tolist()
         out = [matches[b, :n[b]] for b in range(len(n))]
         return out if len(n) > 1 else (out[0][:, :2].cpu().numpy(), out[0][:, 2:].cpu().numpy())
+
+    def _mnn_pairs_f32_device(self, tab, rows: torch.Tensor, tp: torch.Tensor, k_max: int):
+        """xfeat_mnn_match_pairs_f32 on the dense table's descriptors for the (B, 2) int32 device pair table `tp`."""
+        B = tp.shape[0]
+        idx0 = self._empty((B, k_max), torch.int64)
+        idx1 = self._empty((B, k_max), torch.int64)
+        cnt = self._empty((B,), torch.int32)
+        ws = self._workspace(self._lib.xfeat_mnn_pairs_f32_workspace_bytes(B, k_max))
+        with torch.cuda.device(self.dev):
+            _lib.check(self._lib.xfeat_mnn_match_pairs_f32(tab["descriptors"].data_ptr(), rows.data_ptr(), rows.shape[0], k_max,
+                                                           tp.data_ptr(), B, idx0.data_ptr(), idx1.data_ptr(), cnt.data_ptr(),
+                                                           ws.data_ptr(), ws.numel(), self._stream()), "xfeat_mnn_match_pairs_f32")
+        return idx0, idx1, cnt
+
+    def _refine_pairs_device(self, tab, tp: torch.Tensor, idx0, idx1, cnt, k_max: int, fine_conf: float = 0.25):
+        B = tp.shape[0]
+        matches = self._empty((B, k_max, 4))
+        n_ref = self._empty((B,), torch.int32)
+        ws = self._workspace(self._lib.xfeat_refine_pairs_workspace_bytes(B, k_max))
+        with torch.cuda.device(self.dev):
+            _lib.check(self._lib.xfeat_refine_pairs(self._ctx, tab["descriptors"].data_ptr(), tab["keypoints"].data_ptr(),
+                                                    tab["scales"].data_ptr(), k_max, tp.data_ptr(), idx0.data_ptr(),
+                                                    idx1.data_ptr(), cnt.data_ptr(), B, float(fine_conf), matches.data_ptr(),
+                                                    n_ref.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()),
+                       "xfeat_refine_pairs")
+        return matches, n_ref
+
+    @torch.inference_mode()
+    def match_xfeat_star_pairs(self, images, pairs, top_k=None) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """match_xfeat_star over a list of pairs into one set of images (inputs as match_xfeat_pairs): result p is what
+        match_xfeat_star(images[i], images[j], top_k) returns for pairs[p] = (i, j), bit for bit -- self pairs, repeated pairs
+        and both orders included.
+
+        Only images some pair names are extracted, each exactly once per scale, in launch sequences of up to 64 images of one
+        bucket, into one dense table of K_max rows per image.  The pairs are then matched and refined straight from the table, as
+        many per launch as fit in STAR_PAIRS_MATCH_BYTES, with one host synchronisation per chunk.  The matcher splits every pair's
+        operands at the exponent of its own two images' max |x|, as the single-pair call does; under matcher implementations 0
+        and 4 each pair goes through the fp32-input matcher on its two table slots instead."""
+        if top_k is None: top_k = self.top_k
+        keys = [pair_image_key(x) for x in images]
+        plan = PairPlan(keys, pairs, PAIRS_EXTRACT_CHUNK)
+        if len(plan.pairs) == 0:
+            return []
+        rows = star_pair_rows(keys, plan, top_k)                    # refuses a too-small image before anything is launched
+        k_max = int(rows.max())
+        presplit = self._lib.xfeat_get_mnn_impl() in (1, 2, 3)
+        order = plan.match_order()
+        tp_all = torch.from_numpy(np.ascontiguousarray(plan.table_pairs[order])).to(self.dev)
+        rows_dev = torch.from_numpy(rows).to(self.dev)
+        n = plan.n_slots
+        tab = {"keypoints": self._empty((n, k_max, 2)), "descriptors": self._empty((n, k_max, 64)), "scales": self._empty((n, k_max))}
+
+        def step(cur, out):       # one bucket: one shape, dtype and "/255" flag
+            x = cur[0][0] if len(cur) == 1 else torch.cat([t for t, _ in cur])
+            self._dense_device(x, top_k, True, cur[0][1], out=out)
+        self._fill_table(images, plan, tab, step)
+
+        out: List = [None] * len(order)
+        for o0, o1 in star_match_chunks(len(order), k_max):
+            sel, tp = order[o0:o1], tp_all[o0:o1]
+            B = len(sel)
+            if presplit:
+                idx0, idx1, cnt = self._mnn_pairs_f32_device(tab, rows_dev, tp, k_max)
+            else:
+                idx0 = self._empty((B, k_max), torch.int64)
+                idx1 = self._empty((B, k_max), torch.int64)
+                cnt = self._empty((B,), torch.int32)
+                d = tab["descriptors"]
+                for b, (si, sj) in enumerate(plan.table_pairs[sel].tolist()):
+                    ki, kj = int(rows[si]), int(rows[sj])
+                    i0, i1, c = self._mnn_device(d[si], None, ki, ki * 64, d[sj], None, kj, kj * 64, 1, -1)
+                    idx0[b, :ki] = i0[0]
+                    idx1[b, :ki] = i1[0]
+                    cnt[b:b + 1] = c
+            matches, n_ref = self._refine_pairs_device(tab, tp, idx0, idx1, cnt, k_max)
+            hm = torch.empty(matches.shape, dtype=torch.float32, pin_memory=True)
+            hn = torch.empty((B,), dtype=torch.int32, pin_memory=True)
+            hm.copy_(matches, non_blocking=True)
+            hn.copy_(n_ref, non_blocking=True)
+            torch.cuda.current_stream(self.dev).synchronize()         # the only host sync of this chunk
+            c = hn.tolist()
+            m = hm.numpy()
+            for b, p in enumerate(sel.tolist()):
+                out[p] = (m[b, :c[b], :2].copy(), m[b, :c[b], 2:].copy())
+        return out
 
     # ------------------------------------------------------------------------------------------------------------
     # LighterGlue matching (csrc/lighterglue.cu)

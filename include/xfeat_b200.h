@@ -203,6 +203,16 @@ XF_API int xfeat_mnn_match_pairs(const void* d_fs, const int32_t* d_n, int n_ima
 XF_API int xfeat_gather_matches_pairs(const float* d_kpts, int n_max, const int32_t* d_pairs, const int64_t* d_idx0,
                                const int64_t* d_idx1, const int32_t* d_n_matches, int n_pairs,
                                float* d_out0, float* d_out1, void* stream);
+/* Semi-dense pair lists over one fp32 table (XFeat.match_xfeat_star_pairs): d_f (n_images, n_max, 64) un-normalised
+ * descriptors, d_n (n_images) counts, d_pairs (n_pairs, 2) int32 device image indices, each in [0, n_images) (the caller validates
+ * them).  Per pair p = (i, j), at capacity n_max: the result of xfeat_mnn_match on images i and j alone (first d_n[i] / d_n[j]
+ * rows, abs_bound 0, min_cossim -1), bit for bit -- each pair's operands are split at the exponent of max |x| over its own two
+ * images.  Implementations 1-3, XF_E_UNSUPPORTED otherwise; n_pairs * n_pad < 2^31 (n_pad: n_max rounded up to 512);
+ * n_pairs <= 65535. */
+XF_API size_t xfeat_mnn_pairs_f32_workspace_bytes(int n_pairs, int n_max);
+XF_API int xfeat_mnn_match_pairs_f32(const float* d_f, const int32_t* d_n, int n_images, int n_max, const int32_t* d_pairs,
+                              int n_pairs, int64_t* d_idx0, int64_t* d_idx1, int32_t* d_n_matches, void* d_ws,
+                              size_t ws_bytes, void* stream);
 
 XF_API size_t xfeat_refine_workspace_bytes(int batch, int n_max);
 /* replaces: XFeat.refine_matches + fine_matcher + subpix_softmax2d (xfeat.py:292-325, model.py:97-111), for all
@@ -215,6 +225,15 @@ XF_API int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d_des
                  const float* d_kpts1, const float* d_scales0, const int64_t* d_idx0, const int64_t* d_idx1,
                  const int32_t* d_n_matches, int batch, int n_max, int n1_max, float fine_conf, float* d_matches,
                  int32_t* d_n_refined, void* d_ws, size_t ws_bytes, void* stream);
+/* xfeat_refine for pair p = (i, j) of d_pairs (n_pairs, 2) int32 (8-byte aligned): desc0 / kpts0 / scales0 are slot i and
+ * desc1 / kpts1 slot j of one table -- d_desc (n_images, n_max, 64), d_kpts (n_images, n_max, 2), d_scales (n_images, n_max) --
+ * and d_idx0 / d_idx1 (n_pairs, n_max), d_n_matches (n_pairs) come from xfeat_mnn_match_pairs_f32.  Result p equals xfeat_refine
+ * on the two images' own slices, bit for bit. */
+XF_API size_t xfeat_refine_pairs_workspace_bytes(int n_pairs, int n_max);
+XF_API int xfeat_refine_pairs(xfeat_ctx* ctx, const float* d_desc, const float* d_kpts, const float* d_scales, int n_max,
+                       const int32_t* d_pairs, const int64_t* d_idx0, const int64_t* d_idx1, const int32_t* d_n_matches,
+                       int n_pairs, float fine_conf, float* d_matches, int32_t* d_n_refined, void* d_ws, size_t ws_bytes,
+                       void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Stand-alone forms of the reference's helper methods (the same arithmetic runs fused inside the stage entry points)

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Pair-list matching (XFeat.match_xfeat_pairs) against per-batch extraction (match_xfeat_stream), on one GPU.
+"""Pair-list matching (XFeat.match_xfeat_pairs, match_xfeat_star_pairs) against per-batch extraction (match_xfeat_stream,
+match_xfeat_star), on one GPU.
 
 Workloads (sparse, top_k 4096, uint8 numpy images on the host, as the evaluation harness passes them):
   a  MegaDepth-1500 replay: the benchmark's pair structure (tests/golden/megadepth1500_pairs.npz: 806 images in 20 shapes, 1500
@@ -11,6 +12,14 @@ Workloads (sparse, top_k 4096, uint8 numpy images on the host, as the evaluation
   c  512 distinct VGA pairs, no image repeated: match_xfeat_pairs against match_xfeat_stream in 64-pair batches.
   d  the pair order of the matcher launch: xfeat_mnn_match_pairs alone on the extracted tables of (a) and (b), pairs sorted by
      (j, i) against a seeded shuffle.
+Semi-dense (XFeat*), the same synthetic images:
+  e  the MegaDepth-1500 replay at top_k 10 000 (the reference's XFeat* setting; all 20 sizes give 10 000 rows per image): one
+     match_xfeat_star_pairs call against the harness's former star mode, restated here: (shape0, shape1) groups, 64-pair chunks
+     through match_xfeat_star.
+  f  exhaustive matching of 64 VGA images at top_k 4096: one match_xfeat_star_pairs call against the same pairs through
+     match_xfeat_star in 64-pair batches.
+  The batched old arm splits each batch's descriptors at one exponent for the whole batch, so both arms are also compared with
+  per-pair match_xfeat_star calls on a seeded sample of pairs; every pair where an arm differs is listed.
 Every time is CUDA events around the whole call (each call ends with its results on the host); A and B alternate.  The card's
 name and power limit are read in the same run.
 
@@ -81,6 +90,47 @@ def stream_grouped(xf, images, pairs, batch=64):
     return out
 
 
+def star_grouped(xf, images, pairs, top_k, batch=64):
+    """The harness's former star mode: pairs grouped by (shape0, shape1), 64-pair chunks through match_xfeat_star."""
+    out = [None] * len(pairs)
+    groups = {}
+    for p, (i, j) in enumerate(pairs):
+        groups.setdefault((images[i].shape, images[j].shape), []).append(p)
+    for idxs in groups.values():
+        for ch in (idxs[o:o + batch] for o in range(0, len(idxs), batch)):
+            res = xf.match_xfeat_star(np.stack([images[pairs[p][0]] for p in ch]), np.stack([images[pairs[p][1]] for p in ch]),
+                                      top_k=top_k)
+            if len(ch) == 1:
+                out[ch[0]] = res                                  # B == 1: two numpy arrays
+            else:
+                for p, m in zip(ch, res):
+                    m = m.cpu().numpy()
+                    out[p] = (m[:, :2], m[:, 2:])
+    return out
+
+
+def star_workload(xf, name, images, pairs, top_k, reps, sample=48):
+    pair_list = [tuple(p) for p in np.asarray(pairs).tolist()]
+    res, outs = ab(name, {
+        "star_pairs_one_call": lambda: xf.match_xfeat_star_pairs(images, pairs, top_k=top_k),
+        "star_grouped_64": lambda: star_grouped(xf, images, pair_list, top_k),
+    }, reps)
+    sel = np.sort(np.random.default_rng(1).choice(len(pair_list), min(sample, len(pair_list)), replace=False)).tolist()
+    diff = {"star_pairs_one_call": [], "star_grouped_64": []}
+    for p in sel:
+        i, j = pair_list[p]
+        w = xf.match_xfeat_star(images[i], images[j], top_k=top_k)
+        for arm in diff:
+            if not same([outs[arm][p]], [w]):
+                diff[arm].append({"pair": p, "images": [i, j], "n": len(outs[arm][p][0]), "n_single": len(w[0])})
+    res["sample_pairs"] = len(sel)
+    res["differs_from_single_pair_calls"] = diff
+    res["arms_identical"] = same(outs["star_pairs_one_call"], outs["star_grouped_64"])
+    res["matches_total"] = int(sum(len(r[0]) for r in outs["star_pairs_one_call"]))
+    print(name, "differs from single-pair calls:", {k: len(v) for k, v in diff.items()}, flush=True)
+    return res
+
+
 def pairs_chunked(xf, images, pairs, chunk):
     out = []
     for o in range(0, len(pairs), chunk):
@@ -113,7 +163,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", help="also write the JSON result to this file")
-    ap.add_argument("--only", default="abcd")
+    ap.add_argument("--only", default="abcdef")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_pairs needs a GPU")
@@ -124,7 +174,7 @@ def main():
     result = {"card": card(), "top_k": TOPK, "reps": args.reps}
     t0 = time.time()
 
-    if "a" in args.only or "d" in args.only:
+    if any(w in args.only for w in "ade"):
         with np.load(os.path.join(ROOT, "tests", "golden", "megadepth1500_pairs.npz")) as z:
             sizes, md_pairs = z["sizes"], z["pairs"]
         md_images = [synth(ref if k % 2 == 0 else tgt, int(h), int(w), rng) for k, (h, w) in enumerate(sizes)]
@@ -160,6 +210,10 @@ def main():
         res["identical_outputs"] = same(outs["pairs_one_call"], outs["stream_64"])
         result["c_uniform512"] = res
         del uni
+    if "e" in args.only:
+        result["e_star_megadepth1500"] = star_workload(xf, "e_star_megadepth", md_images, md_pairs, 10_000, args.reps)
+    if "f" in args.only:
+        result["f_star_exhaustive64"] = star_workload(xf, "f_star_exhaustive", vga, ex_pairs, 4096, args.reps)
     if "d" in args.only:
         result["d_order"] = {"megadepth1500": order_effect(xf, md_images, md_pairs, 3 * args.reps),
                              "exhaustive64": order_effect(xf, vga, ex_pairs, 3 * args.reps)}
