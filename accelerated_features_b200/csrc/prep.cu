@@ -520,6 +520,14 @@ extern "C" int xfeat_preprocess_scaled(const void* d_img, int dtype, int B, int 
     (void)cudaGetLastError();      // a refused cluster shape is a launch-configuration error: nothing ran, try the next form
     cluster_cap = cl == 16 ? 8 : 0;
     cluster_cap_a.store(cluster_cap, std::memory_order_relaxed);
+    // Inside a stream capture the refused launch has already invalidated the capture, so a retry cannot rescue it: report the
+    // refusal.  The step-down above is kept, so the same call made outside a capture takes the smaller form from then on.
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+      xf::set_error("preprocess: cluster launch of %d CTAs refused (%s) during a stream capture; run the call once before "
+                    "capturing it", cl, cudaGetErrorString(e));
+      return XF_E_CUDA;
+    }
   }
   if (fast_u8) {
     dim3 g4(xf::cdiv(W / 4, 64), xf::cdiv(H, 4), B);

@@ -13,10 +13,13 @@ from . import _lib
 
 
 def find_homography_batch(pts0: torch.Tensor, pts1: torch.Tensor, counts: Optional[torch.Tensor] = None, thr: float = 3.0,
-                          iters: int = 1024, seed: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                          iters: int = 1024, seed: int = 0,
+                          workspace: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """pts0, pts1: (B, n_max, 2) float32 CUDA tensors of matched coordinates (pair b uses the first counts[b] rows; None: all).
     Returns H (B,3,3) float32 with H[2,2] = 1 mapping image-0 to image-1 pixels, inliers (B, n_max) bool, n_inliers (B) int32.
-    `thr`: forward transfer error in pixels of image 1 (cv2's ransacReprojThreshold)."""
+    `thr`: forward transfer error in pixels of image 1 (cv2's ransacReprojThreshold).  `workspace`: a uint8 CUDA tensor of at
+    least xfeat_ransac_workspace_bytes(B, iters) bytes to use as scratch (default: a fresh one), for callers that capture the
+    call into a CUDA graph and keep the scratch alive with it."""
     lib = _lib.load()
     if not (pts0.is_cuda and pts1.is_cuda):
         raise RuntimeError("find_homography_batch runs on the GPU only (no CPU fallback)")
@@ -32,7 +35,9 @@ def find_homography_batch(pts0: torch.Tensor, pts1: torch.Tensor, counts: Option
     if B == 0 or n_max == 0:
         return H, mask.bool(), n_inl
     cnt = None if counts is None else counts.to(dev).to(torch.int32).contiguous()
-    ws = torch.empty(max(256, lib.xfeat_ransac_workspace_bytes(B, iters)), dtype=torch.uint8, device=dev)
+    ws = workspace
+    if ws is None:
+        ws = torch.empty(max(256, lib.xfeat_ransac_workspace_bytes(B, iters)), dtype=torch.uint8, device=dev)
     with torch.cuda.device(dev):
         _lib.check(lib.xfeat_ransac_homography(p0.data_ptr(), p1.data_ptr(), None if cnt is None else cnt.data_ptr(), n_max, B,
                                                float(thr), int(iters), int(seed) & 0xffffffff, H.data_ptr(), mask.data_ptr(),

@@ -9,7 +9,8 @@ Beyond the reference surface: `match_xfeat_batch` (batched match_xfeat) and `mat
 host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match_lighterglue_batch` and
 `match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu), `match_xfeat_pairs` and
 `match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once), and
-`match_xfeat_star_pairs` (the same for semi-dense matching: XFeat* over a list of pairs, each image extracted once per scale).
+`match_xfeat_star_pairs` (the same for semi-dense matching: XFeat* over a list of pairs, each image extracted once per scale),
+and `tracker` (one reference tracked through a video stream, each frame's step replayed as one CUDA graph; tracker.py).
 """
 from __future__ import annotations
 
@@ -355,13 +356,15 @@ class XFeat(torch.nn.Module):
                            "xfeat_preprocess_scaled")
         return xn
 
-    def _run_net(self, xn: torch.Tensor, B: int, H: int, W: int, want_logits: bool = False):
+    def _run_net(self, xn: torch.Tensor, B: int, H: int, W: int, want_logits: bool = False, ws: Optional[torch.Tensor] = None):
+        """`ws`: scratch to use instead of the instance's per-stream workspace (a caller that captures the call into a CUDA graph
+        passes one it owns, so that a later eager call growing the instance's workspace cannot free memory the graph reads)."""
         feats = self._empty((B, H // 8, W // 8, 64))
         heat = self._empty((B, H, W))
         rel = self._empty((B, H // 8, W // 8))
         logits = self._empty((B, H // 8, W // 8, 65)) if want_logits else None
-        nbytes = self._lib.xfeat_net_workspace_bytes(B, H, W)
-        ws = self._workspace(nbytes)
+        if ws is None:
+            ws = self._workspace(self._lib.xfeat_net_workspace_bytes(B, H, W))
         with torch.cuda.device(self.dev):
             _lib.check(self._lib.xfeat_net(self._ctx, xn.data_ptr(), B, H, W, feats.data_ptr(), heat.data_ptr(),
                                            rel.data_ptr(), _ptr(logits), ws.data_ptr(), ws.numel(), self._stream()),
@@ -389,13 +392,15 @@ class XFeat(torch.nn.Module):
         return (top_k + 511) // 512 * 512                       # row padding of the tensor-core matcher (mnn_tc.cu)
 
     def _detect_sparse_device(self, x, top_k: int, detection_threshold: float, div255=False, want_split: bool = False,
-                              want_desc: bool = True, out: Optional[Dict[str, torch.Tensor]] = None):
+                              want_desc: bool = True, out: Optional[Dict[str, torch.Tensor]] = None,
+                              ws: Optional[torch.Tensor] = None):
         """Whole sparse extraction on the device, fixed-capacity outputs, no host sync.  `x` is one image batch or a list
         of batches of identical shape (they are normalised into one activation batch without concatenating the inputs);
         `div255` is one flag or one per batch (parse_input's "/255" applies to numpy inputs only, xfeat.py:400-401).
         `want_split`: also return 'desc_split' (B, split_rows, 128) fp16, the matcher's pre-split operand rows.
         `out`: write 'keypoints', 'n_valid' and (when asked for) 'descriptors' / 'desc_split' into these (B, ...) tensors, e.g.
         slices of an image table, instead of fresh ones.
+        `ws`: scratch for the network and the selection instead of the instance's workspace (see _run_net).
         Returns dict of device tensors: keypoints (B,k,2), scores (B,k), descriptors (B,k,64), n_valid (B) int32."""
         xs = [self._to_bchw(t) for t in (x if isinstance(x, (list, tuple)) else [x])]
         flags = list(div255) if isinstance(div255, (list, tuple)) else [div255] * len(xs)
@@ -416,7 +421,10 @@ class XFeat(torch.nn.Module):
         for t, f in zip(xs, flags):
             self._preprocess(t, H, W, bool(f), out=xn[o:o + t.shape[0]])
             o += t.shape[0]
-        feats, heat, rel, _ = self._run_net(xn, B, H, W)
+        if ws is None:
+            feats, heat, rel, _ = self._run_net(xn, B, H, W)
+        else:
+            feats, heat, rel, _ = self._run_net(xn, B, H, W, ws=ws)
         dst = out or {}
         kpts = dst["keypoints"] if "keypoints" in dst else self._empty((B, top_k, 2))
         scores = self._empty((B, top_k))
@@ -428,7 +436,8 @@ class XFeat(torch.nn.Module):
         nbytes = self._lib.xfeat_sparse_workspace_bytes(B, H, W, top_k)
         if nbytes == 0:
             raise _lib.XFeatLibraryError("xfeat_sparse_workspace_bytes failed: " + self._lib.xfeat_last_error().decode())
-        ws = self._workspace(nbytes)
+        if ws is None:
+            ws = self._workspace(nbytes)
         split_rows = self._split_rows(top_k)
         split = None
         if want_split:
@@ -458,13 +467,14 @@ class XFeat(torch.nn.Module):
         return [{"keypoints": out["keypoints"][b, :n[b]], "scores": out["scores"][b, :n[b]],
                  "descriptors": out["descriptors"][b, :n[b]]} for b in range(len(n))]
 
-    def _mnn_device(self, f1, n1, n1_max, stride1, f2, n2, n2_max, stride2, batch, min_cossim, abs_bound=0.0):
+    def _mnn_device(self, f1, n1, n1_max, stride1, f2, n2, n2_max, stride2, batch, min_cossim, abs_bound=0.0, ws=None):
         """abs_bound > 0: the caller guarantees max|f| <= abs_bound (1.0 for the sparse path's unit-norm descriptors), which
-        spares the tensor-core matcher its max-reduction pass over both descriptor sets."""
+        spares the tensor-core matcher its max-reduction pass over both descriptor sets.  `ws`: see _run_net."""
         idx0 = self._empty((batch, n1_max), torch.int64)
         idx1 = self._empty((batch, n1_max), torch.int64)
         cnt = self._empty((batch,), torch.int32)
-        ws = self._workspace(self._lib.xfeat_mnn_workspace_bytes(batch, n1_max, n2_max))
+        if ws is None:
+            ws = self._workspace(self._lib.xfeat_mnn_workspace_bytes(batch, n1_max, n2_max))
         with torch.cuda.device(self.dev):
             _lib.check(self._lib.xfeat_mnn_match_bounded(f1.data_ptr(), _ptr(n1), n1_max, stride1, f2.data_ptr(), _ptr(n2),
                                                          n2_max, stride2, batch, float(min_cossim), float(abs_bound),
@@ -593,6 +603,15 @@ class XFeat(torch.nn.Module):
         self._check_counts(c, "match_xfeat_verified_batch")
         mk0, mk1, H, mask = mk0.cpu().numpy(), mk1.cpu().numpy(), H.cpu().numpy(), mask.cpu().numpy()
         return [{"mkpts0": mk0[b, :c[b]], "mkpts1": mk1[b, :c[b]], "H": H[b], "inliers": mask[b, :c[b]]} for b in range(len(c))]
+
+    def tracker(self, reference, top_k=None, min_cossim: float = 0.82, ransac_thr: float = 4.0, iters: int = 700,
+                min_inliers: int = 50, seed: int = 0):
+        """A Tracker (tracker.py) of `reference` through a video stream: per frame, match_xfeat(reference, frame, top_k,
+        min_cossim) and the homography RANSAC of match_xfeat_verified_batch, replayed as one CUDA graph per frame shape with the
+        reference extracted once.  The defaults are realtime_demo.py's (min_cossim 0.82, USAC_MAGSAC at 4 px, 700 iterations,
+        homographies with fewer than 50 inliers dropped).  top_k above 8192 is refused."""
+        from .tracker import Tracker
+        return Tracker(self, reference, top_k, min_cossim, ransac_thr, iters, min_inliers, seed)
 
     # ------------------------------------------------------------------------------------------------------------
     # streaming: pinned, double-buffered host -> device -> host pipeline (SURVEY 8f-1)
@@ -787,20 +806,43 @@ class XFeat(torch.nn.Module):
             cur, s0 = nxt, s1
         return tab
 
-    def _mnn_pairs_device(self, tab, tp: torch.Tensor, top_k: int, min_cossim: float):
-        """xfeat_mnn_match_pairs on the table's operand rows for the (B, 2) int32 device pair table `tp`."""
+    def _mnn_pairs_device(self, tab, tp: torch.Tensor, top_k: int, min_cossim: float, ws: Optional[torch.Tensor] = None):
+        """xfeat_mnn_match_pairs on the table's operand rows for the (B, 2) int32 device pair table `tp`.  `ws`: see _run_net."""
         B = tp.shape[0]
         sp = tab["desc_split"]
         idx0 = self._empty((B, top_k), torch.int64)
         idx1 = self._empty((B, top_k), torch.int64)
         cnt = self._empty((B,), torch.int32)
-        ws = self._workspace(self._lib.xfeat_mnn_pairs_workspace_bytes(B, top_k))
+        if ws is None:
+            ws = self._workspace(self._lib.xfeat_mnn_pairs_workspace_bytes(B, top_k))
         with torch.cuda.device(self.dev):
             _lib.check(self._lib.xfeat_mnn_match_pairs(sp.data_ptr(), tab["n_valid"].data_ptr(), sp.shape[0], top_k, sp.shape[1],
                                                        tp.data_ptr(), B, 13, float(min_cossim), idx0.data_ptr(), idx1.data_ptr(),
                                                        cnt.data_ptr(), ws.data_ptr(), ws.numel(), self._stream()),
                        "xfeat_mnn_match_pairs")
         return idx0, idx1, cnt
+
+    def _match_table_pairs(self, tab, tp: torch.Tensor, top_k: int, min_cossim: float, presplit: bool,
+                           ws: Optional[torch.Tensor] = None):
+        """MNN + keypoint gather of the (B, 2) int32 device pair table `tp` over an _extract_table table: xfeat_mnn_match_pairs
+        on its operand rows (`presplit`), else xfeat_mnn_match_bounded on its fp32 descriptors gathered per pair.  Returns mkpts0,
+        mkpts1 (B, top_k, 2) and n_matches (B) int32 (XF_N_OVERFLOW for a pair with an overflowed image).  No host sync.
+        `ws`: see _run_net."""
+        B = tp.shape[0]
+        if presplit:
+            idx0, idx1, cnt = self._mnn_pairs_device(tab, tp, top_k, min_cossim, ws=ws)
+        else:
+            ti, tj = tp[:, 0].long(), tp[:, 1].long()
+            d, n = tab["descriptors"], tab["n_valid"]
+            idx0, idx1, cnt = self._mnn_device(d.index_select(0, ti), n.index_select(0, ti), top_k, top_k * 64,
+                                               d.index_select(0, tj), n.index_select(0, tj), top_k, top_k * 64, B, min_cossim,
+                                               abs_bound=1.0, ws=ws)
+        mk0, mk1 = self._empty((B, top_k, 2)), self._empty((B, top_k, 2))
+        with torch.cuda.device(self.dev):
+            _lib.check(self._lib.xfeat_gather_matches_pairs(tab["keypoints"].data_ptr(), top_k, tp.data_ptr(), idx0.data_ptr(),
+                                                            idx1.data_ptr(), cnt.data_ptr(), B, mk0.data_ptr(), mk1.data_ptr(),
+                                                            self._stream()), "xfeat_gather_matches_pairs")
+        return mk0, mk1, cnt
 
     @staticmethod
     def _pair_labels(plan: PairPlan, sel: np.ndarray) -> List[str]:
@@ -828,19 +870,7 @@ class XFeat(torch.nn.Module):
         for o in range(0, len(order), step):
             sel, tp = order[o:o + step], tp_all[o:o + step]
             B = len(sel)
-            if presplit:
-                idx0, idx1, cnt = self._mnn_pairs_device(tab, tp, top_k, min_cossim)
-            else:
-                ti, tj = tp[:, 0].long(), tp[:, 1].long()
-                d, n = tab["descriptors"], tab["n_valid"]
-                idx0, idx1, cnt = self._mnn_device(d.index_select(0, ti), n.index_select(0, ti), top_k, top_k * 64,
-                                                   d.index_select(0, tj), n.index_select(0, tj), top_k, top_k * 64, B, min_cossim,
-                                                   abs_bound=1.0)
-            mk0, mk1 = self._empty((B, top_k, 2)), self._empty((B, top_k, 2))
-            with torch.cuda.device(self.dev):
-                _lib.check(self._lib.xfeat_gather_matches_pairs(tab["keypoints"].data_ptr(), top_k, tp.data_ptr(), idx0.data_ptr(),
-                                                                idx1.data_ptr(), cnt.data_ptr(), B, mk0.data_ptr(),
-                                                                mk1.data_ptr(), self._stream()), "xfeat_gather_matches_pairs")
+            mk0, mk1, cnt = self._match_table_pairs(tab, tp, top_k, min_cossim, presplit)
             h0, h1 = (torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (mk0, mk1))
             hc = torch.empty((B,), dtype=torch.int32, pin_memory=True)
             for h, t in ((h0, mk0), (h1, mk1), (hc, cnt)):

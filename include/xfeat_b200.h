@@ -13,6 +13,19 @@
  *   - activations are channels-last (NHWC) fp32; the dense feature map returned to the caller is
  *     (B, H/8, W/8, 64) channels-last, the keypoint heat-map is (B, H, W), reliability is (B, H/8, W/8);
  *   - H, W below are the network resolution: multiples of 32 (xfeat.py:235-236).
+ *
+ * CUDA-graph capture
+ *   xfeat_preprocess(_scaled), xfeat_net, xfeat_detect_sparse(_split), xfeat_mnn_match(_bounded), xfeat_mnn_match_presplit,
+ *   xfeat_mnn_match_pairs, xfeat_gather_matches(_pairs) and xfeat_ransac_homography may be called on a stream under capture
+ *   (cudaStreamBeginCapture, any mode).  They enqueue kernels, cudaMemsetAsync and device-to-device cudaMemcpyAsync only; they
+ *   never synchronise, allocate, or read device memory on the host; every buffer they touch is a caller pointer or a slice of
+ *   the caller's workspace, so the captured graph stays valid for as long as the caller keeps those buffers (and their size)
+ *   unchanged.  Host-side decisions are frozen into the graph at capture: the matcher implementation (xfeat_set_mnn_impl),
+ *   the convolution implementation (xfeat_set_conv_impl) and the XFEAT_* environment switches.  One condition: make each
+ *   call once, with the same shapes, outside a capture before capturing it.  That first call settles what the library decides
+ *   on first use -- the dynamic shared-memory opt-ins, the tensor-map encoder lookup, and xfeat_preprocess's cluster size,
+ *   which steps down 16 -> 8 -> two kernels when the device refuses a cluster launch.  A refused launch invalidates a capture,
+ *   so under capture xfeat_preprocess reports the refusal (XF_E_CUDA) instead of retrying.
  */
 #ifndef XFEAT_B200_H
 #define XFEAT_B200_H
