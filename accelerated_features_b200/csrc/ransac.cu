@@ -6,7 +6,8 @@
 //   hypothesise from minimal samples -> score every hypothesis on all correspondences -> keep the best -> re-fit on its
 //   inliers (local optimisation) -> classify with the threshold,
 // with MSAC scoring (truncated squared error).  Parity is anchored on the call sites: same inputs, same threshold meaning
-// (pixels of the second image for the homography, Sampson distance in normalised image coordinates for the essential matrix);
+// (pixels of the second image for the homography, Sampson distance in normalised image coordinates for the essential matrix,
+// Sampson distance in pixels for the fundamental matrix as in OpenCV's USAC methods);
 // tests compare inlier sets and model error with cv2 on the same correspondences (stochastic: agreement, not bit equality).
 //
 // One launch scores ALL hypotheses of ALL pairs: a block caches the (Hartley-normalised) correspondences of its pair in
@@ -87,10 +88,10 @@ __device__ bool rs_solve_h4(const float (&x)[4], const float (&y)[4], const floa
   return true;
 }
 
-// Smallest-eigenvalue eigenvector of a symmetric N x N matrix (cyclic Jacobi, fp64); M is destroyed.
+// Eigen-decomposition of a symmetric N x N matrix (cyclic Jacobi, fp64): M is diagonalised in place (eigenvalue i on M[i][i]),
+// the eigenvectors are the columns of V.
 template <int N>
-__device__ void rs_smallest_eigvec(double (&M)[N][N], double (&vec)[N]) {
-  double V[N][N];
+__device__ __forceinline__ void rs_jacobi(double (&M)[N][N], double (&V)[N][N]) {
   for (int i = 0; i < N; ++i)
     for (int j = 0; j < N; ++j) V[i][j] = (i == j) ? 1.0 : 0.0;
   for (int sweep = 0; sweep < 30; ++sweep) {
@@ -121,6 +122,13 @@ __device__ void rs_smallest_eigvec(double (&M)[N][N], double (&vec)[N]) {
         }
       }
   }
+}
+
+// Smallest-eigenvalue eigenvector of a symmetric N x N matrix (cyclic Jacobi, fp64); M is destroyed.
+template <int N>
+__device__ void rs_smallest_eigvec(double (&M)[N][N], double (&vec)[N]) {
+  double V[N][N];
+  rs_jacobi<N>(M, V);
   int best = 0;
   for (int i = 1; i < N; ++i)
     if (M[i][i] < M[best][best]) best = i;
@@ -408,6 +416,22 @@ __device__ __forceinline__ void rs_epi_row(float x, float y, float u, float v, d
   r[0] = (double)u * x; r[1] = (double)u * y; r[2] = u; r[3] = (double)v * x; r[4] = (double)v * y; r[5] = v; r[6] = x; r[7] = y; r[8] = 1.0;
 }
 
+// Nearest rank-2 matrix in the Frobenius norm: F - (F v) v^T with v the right singular vector of the smallest singular value
+// (the eigenvector of F^T F of its smallest eigenvalue).
+__device__ void rs_project_rank2(double (&F)[9]) {
+  double M[3][3], V[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) M[i][j] = F[0 + i] * F[0 + j] + F[3 + i] * F[3 + j] + F[6 + i] * F[6 + j];
+  rs_jacobi<3>(M, V);
+  int lo = 0;
+  for (int i = 1; i < 3; ++i)
+    if (M[i][i] < M[lo][lo]) lo = i;
+  for (int r = 0; r < 3; ++r) {
+    const double w = F[3 * r] * V[0][lo] + F[3 * r + 1] * V[1][lo] + F[3 * r + 2] * V[2][lo];
+    for (int k = 0; k < 3; ++k) F[3 * r + k] -= w * V[k][lo];
+  }
+}
+
 __global__ void __launch_bounds__(RS_THREADS) ransac_e_hyp_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
                                                                   const int* __restrict__ np, int n_max, float thr,
                                                                   int rounds_per_warp, uint32_t seed, RsRecord* __restrict__ best) {
@@ -491,11 +515,12 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_e_hyp_kernel(const float* _
 // one IRLS step towards the Sampson error) over the points within mult*thr of the current model, mult shrinking 3 -> 1.  The model
 // kept is the one with the lowest MSAC cost at the true threshold, so the result is never worse than the candidate.
 // sE (shared, 9 floats): candidate in, optimised model out (visible to all threads on return).  Returns its MSAC cost.
-__device__ float rs_e_local_opt(const float4* __restrict__ sPts, int n, float t2, float* sE) {
-  __shared__ double sAcc[RS_WARPS][45];
-  __shared__ float sCost[RS_WARPS];
-  __shared__ float sBestE[9];
-  __shared__ int sCnt;
+// kRank2: each refit is projected to rank 2 (a fundamental matrix) instead of onto the essential manifold.  The block's shared
+// scratch comes from the caller (rs_e_local_opt / rs_f_local_opt), one set per kernel.
+template <bool kRank2>
+__device__ __forceinline__ float rs_local_opt(const float4* __restrict__ sPts, int n, float t2, float* sE,
+                                              double (&sAcc)[RS_WARPS][45], float (&sCost)[RS_WARPS], float (&sBestE)[9],
+                                              int& sCnt) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float best_cost = 3.0e38f;                         // block-uniform
   __syncthreads();
@@ -566,7 +591,8 @@ __device__ float rs_e_local_opt(const float4* __restrict__ sPts, int n, float t2
           ++e;
         }
       rs_smallest_eigvec<9>(M, vec);
-      rs_project_essential(vec);
+      if constexpr (kRank2) rs_project_rank2(vec);
+      else rs_project_essential(vec);
       for (int k = 0; k < 9; ++k) sE[k] = (float)vec[k];
     }
     __syncthreads();
@@ -575,6 +601,22 @@ __device__ float rs_e_local_opt(const float4* __restrict__ sPts, int n, float t2
   if (threadIdx.x < 9) sE[threadIdx.x] = sBestE[threadIdx.x];
   __syncthreads();
   return best_cost;
+}
+
+__device__ float rs_e_local_opt(const float4* __restrict__ sPts, int n, float t2, float* sE) {
+  __shared__ double sAcc[RS_WARPS][45];
+  __shared__ float sCost[RS_WARPS];
+  __shared__ float sBestE[9];
+  __shared__ int sCnt;
+  return rs_local_opt<false>(sPts, n, t2, sE, sAcc, sCost, sBestE, sCnt);
+}
+
+__device__ float rs_f_local_opt(const float4* __restrict__ sPts, int n, float t2, float* sF) {
+  __shared__ double sAcc[RS_WARPS][45];
+  __shared__ float sCost[RS_WARPS];
+  __shared__ float sBestF[9];
+  __shared__ int sCnt;
+  return rs_local_opt<true>(sPts, n, t2, sF, sAcc, sCost, sBestF, sCnt);
 }
 
 // stage 2: every block's winner is optimised on its own (grid (blocks_per_pair, batch)) -- with w^8 all-inlier samples the raw
@@ -650,6 +692,245 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_e_final_kernel(const float*
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Fundamental matrix (uncalibrated two-view geometry; what cv2.findFundamentalMat(p0, p1, cv2.USAC_*, thr) computes).  Inputs
+// are PIXELS.  Every lane solves one 7-point sample in fp64 (1-3 candidates), the warp scores them with MSAC on the Sampson
+// distance, every block's winner is locally optimised (rs_f_local_opt), and the essential path's final launch classifies
+// with the de-normalised pixel F.  thr is the USAC meaning: Sampson distance in pixels (OpenCV 4.13's USAC_DEFAULT /
+// USAC_ACCURATE / USAC_MAGSAC masks are exactly `Sampson < thr`).
+// ---------------------------------------------------------------------------------------------------------------------
+
+// Normalisation of one pair: each image's centroid to the origin and ONE scale s for both images (mean distance sqrt(2) over
+// all 2n points).  With one scale, the Sampson distance of the normalised points is exactly s times the pixel one, so the pixel
+// threshold thr is thr * s in the normalised frame.  Writes the normalised (x, y, u, v) to sPts, visible to the block on return.
+struct RsPairNorm { float cx0, cy0, cx1, cy1, s; };
+
+__device__ RsPairNorm rs_pair_normalise(const float* __restrict__ q0, const float* __restrict__ q1, int n, float4* sPts,
+                                        float* red /* >= 4 * RS_WARPS floats */) {
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  float a[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int i = threadIdx.x; i < n; i += RS_THREADS) { a[0] += q0[2 * i]; a[1] += q0[2 * i + 1]; a[2] += q1[2 * i]; a[3] += q1[2 * i + 1]; }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    for (int o = 16; o > 0; o >>= 1) a[k] += __shfl_xor_sync(0xffffffffu, a[k], o);
+    if (l == 0) red[k * RS_WARPS + w] = a[k];
+  }
+  __syncthreads();
+  float c[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    for (int i = 0; i < RS_WARPS; ++i) c[k] += red[k * RS_WARPS + i];
+    c[k] /= (float)n;
+  }
+  __syncthreads();
+  float sd = 0.f;
+  for (int i = threadIdx.x; i < n; i += RS_THREADS) {
+    const float dx0 = q0[2 * i] - c[0], dy0 = q0[2 * i + 1] - c[1], dx1 = q1[2 * i] - c[2], dy1 = q1[2 * i + 1] - c[3];
+    sd += sqrtf(dx0 * dx0 + dy0 * dy0) + sqrtf(dx1 * dx1 + dy1 * dy1);
+  }
+  for (int o = 16; o > 0; o >>= 1) sd += __shfl_xor_sync(0xffffffffu, sd, o);
+  if (l == 0) red[w] = sd;
+  __syncthreads();
+  float md = 0.f;
+  for (int i = 0; i < RS_WARPS; ++i) md += red[i];
+  md /= (float)(2 * n);
+  const float s = (md > 1e-12f) ? 1.41421356f / md : 1.f;
+  for (int i = threadIdx.x; i < n; i += RS_THREADS)
+    sPts[i] = make_float4((q0[2 * i] - c[0]) * s, (q0[2 * i + 1] - c[1]) * s, (q1[2 * i] - c[2]) * s, (q1[2 * i + 1] - c[3]) * s);
+  __syncthreads();
+  return RsPairNorm{c[0], c[1], c[2], c[3], s};
+}
+
+__device__ __forceinline__ double rs_det3(const double (&F)[9]) {
+  return F[0] * (F[4] * F[8] - F[5] * F[7]) - F[1] * (F[3] * F[8] - F[5] * F[6]) + F[2] * (F[3] * F[7] - F[4] * F[6]);
+}
+
+// The 7-point solver.  (F1, F2) span the null space of the sample's seven epipolar rows; F = l F1 + (1 - l) F2 with det F = 0 is
+// a cubic in l, whose coefficients come from det F at l = 0, 1, -1, 2.  Each real root (Newton-polished) gives one candidate,
+// scaled to unit Frobenius norm.  Returns the number of candidates (0 for a degenerate sample) written to Fc.
+__device__ int rs_seven_point(const double (&F1)[9], const double (&F2)[9], float (&Fc)[3][9]) {
+  double G[9], p[4];
+  const double at[4] = {0.0, 1.0, -1.0, 2.0};
+  for (int j = 0; j < 4; ++j) {
+    for (int k = 0; k < 9; ++k) G[k] = at[j] * F1[k] + (1.0 - at[j]) * F2[k];
+    p[j] = rs_det3(G);
+  }
+  const double c0 = p[0], c2 = 0.5 * (p[1] + p[2]) - p[0], odd = 0.5 * (p[1] - p[2]);
+  const double c3 = (p[3] - 4.0 * c2 - c0 - 2.0 * odd) / 6.0, c1 = odd - c3;
+  const double cm = fmax(fmax(fabs(c0), fabs(c1)), fmax(fabs(c2), fabs(c3)));
+  if (!(cm > 1e-300)) return 0;
+  double r[3];
+  int nr = 0;
+  if (fabs(c3) > 1e-10 * cm) {                      // l^3 + A l^2 + B l + C; l = t - A/3: t^3 + pp t + qq = 0
+    const double A = c2 / c3, B = c1 / c3, C = c0 / c3;
+    const double pp = B - A * A / 3.0, qq = 2.0 * A * A * A / 27.0 - A * B / 3.0 + C;
+    const double D = 0.25 * qq * qq + pp * pp * pp / 27.0;
+    if (D > 0.0) {
+      const double sD = sqrt(D);
+      r[nr++] = cbrt(-0.5 * qq + sD) + cbrt(-0.5 * qq - sD) - A / 3.0;
+    } else if (pp < 0.0) {
+      const double m = 2.0 * sqrt(-pp / 3.0);
+      const double th = acos(fmin(1.0, fmax(-1.0, 3.0 * qq / (pp * m)))) / 3.0;
+      for (int k = 0; k < 3; ++k) r[nr++] = m * cos(th - 2.0943951023931957 * k) - A / 3.0;
+    } else {
+      r[nr++] = -A / 3.0;
+    }
+  } else if (fabs(c2) > 1e-10 * cm) {               // the cubic term vanishes: the third root is at infinity (F1 - F2)
+    const double disc = c1 * c1 - 4.0 * c2 * c0;
+    if (disc >= 0.0) {
+      const double qd = -0.5 * (c1 + (c1 >= 0.0 ? sqrt(disc) : -sqrt(disc)));
+      r[nr++] = qd / c2;
+      if (qd != 0.0) r[nr++] = c0 / qd;
+    }
+  } else if (fabs(c1) > 1e-10 * cm) {
+    r[nr++] = -c0 / c1;
+  }
+  int nc = 0;
+  for (int j = 0; j < nr; ++j) {
+    double l = r[j];
+    for (int it = 0; it < 2; ++it) {
+      const double f = ((c3 * l + c2) * l + c1) * l + c0, df = (3.0 * c3 * l + 2.0 * c2) * l + c1;
+      if (fabs(df) > 1e-300) l -= f / df;
+    }
+    double nrm = 0.0;
+    for (int k = 0; k < 9; ++k) { G[k] = l * F1[k] + (1.0 - l) * F2[k]; nrm += G[k] * G[k]; }
+    if (!(nrm > 1e-300) || !isfinite(nrm)) continue;
+    const double inv = 1.0 / sqrt(nrm);
+    for (int k = 0; k < 9; ++k) Fc[nc][k] = (float)(G[k] * inv);
+    ++nc;
+  }
+  return nc;
+}
+
+// stage 1: grid (blocks_per_pair, batch).  Samples come from a hash of (seed, pair id, hypothesis id): with the id fixed, a
+// pair's result does not depend on the batch it is in.
+__global__ void __launch_bounds__(RS_THREADS) ransac_f_hyp_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
+                                                                  const int* __restrict__ np, const int* __restrict__ pair_ids,
+                                                                  int n_max, float thr, int rounds_per_warp, uint32_t seed,
+                                                                  RsRecord* __restrict__ best) {
+  extern __shared__ float4 sPts[];                 // (x, y, u, v) normalised (rs_pair_normalise)
+  __shared__ float red[4 * RS_WARPS];
+  __shared__ RsRecord sBest[RS_WARPS];
+  const int pair = blockIdx.y;
+  const int n = min(np ? np[pair] : n_max, min(n_max, RS_MAX_PTS));
+  RsRecord mine;
+  mine.cost = 3.0e38f;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) mine.m[k] = 0.f;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (n >= 8) {
+    const RsPairNorm nz = rs_pair_normalise(p0 + (int64_t)pair * n_max * 2, p1 + (int64_t)pair * n_max * 2, n, sPts, red);
+    const float t2 = (thr * nz.s) * (thr * nz.s);
+    const uint32_t pid = pair_ids ? (uint32_t)pair_ids[pair] : (uint32_t)pair;
+    for (int rd = 0; rd < rounds_per_warp; ++rd) {
+      // every lane: one 7-point sample
+      const uint32_t hid = (uint32_t)(((blockIdx.x * RS_WARPS + warp) * rounds_per_warp + rd) * 32 + lane);
+      uint32_t s = rs_hash(seed ^ (0x9e3779b9u * (pid + 1)) ^ (0x85ebca6bu * (hid + 1)));
+      int idx[7];
+      for (int k = 0; k < 7; ++k) {
+        bool dup;
+        do {
+          s = rs_hash(s + 0x6d2b79f5u);
+          idx[k] = (int)(((uint64_t)s * (uint64_t)n) >> 32);
+          dup = false;
+          for (int j = 0; j < k; ++j) dup |= (idx[j] == idx[k]);
+        } while (dup);
+      }
+      double M[9][9];
+      for (int a = 0; a < 9; ++a)
+        for (int b2 = 0; b2 < 9; ++b2) M[a][b2] = 0.0;
+      for (int k = 0; k < 7; ++k) {
+        const float4 c = sPts[idx[k]];
+        double r[9];
+        rs_epi_row(c.x, c.y, c.z, c.w, r);
+        for (int a = 0; a < 9; ++a)
+          for (int b2 = a; b2 < 9; ++b2) M[a][b2] += r[a] * r[b2];
+      }
+      for (int a = 0; a < 9; ++a)
+        for (int b2 = 0; b2 < a; ++b2) M[a][b2] = M[b2][a];
+      double V[9][9];
+      rs_jacobi<9>(M, V);
+      int i1 = 0, i2 = 1;                           // the two smallest eigenvalues: the null space of the 7 x 9 system
+      if (M[i2][i2] < M[i1][i1]) { i1 = 1; i2 = 0; }
+      for (int i = 2; i < 9; ++i) {
+        if (M[i][i] < M[i1][i1]) { i2 = i1; i1 = i; }
+        else if (M[i][i] < M[i2][i2]) i2 = i;
+      }
+      double F1[9], F2[9];
+      for (int k = 0; k < 9; ++k) { F1[k] = V[k][i1]; F2[k] = V[k][i2]; }
+      float Fc[3][9];
+      const int nc = rs_seven_point(F1, F2, Fc);
+      // the warp scores the lanes' candidates (up to 96) one after the other
+      for (int src = 0; src < 32; ++src) {
+        const int ncs = __shfl_sync(0xffffffffu, nc, src);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          if (j >= ncs) break;
+          float F[9];
+#pragma unroll
+          for (int k = 0; k < 9; ++k) F[k] = __shfl_sync(0xffffffffu, Fc[j][k], src);
+          float cost = 0.f;
+          for (int i = lane; i < n; i += 32) {
+            const float4 c = sPts[i];
+            cost += fminf(rs_sampson2(F, c.x, c.y, c.z, c.w), t2);
+          }
+          for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
+          if (cost < mine.cost) {
+            mine.cost = cost;
+#pragma unroll
+            for (int k = 0; k < 9; ++k) mine.m[k] = F[k];
+          }
+        }
+      }
+    }
+  }
+  if (lane == 0) sBest[warp] = mine;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    RsRecord b = sBest[0];
+    for (int w = 1; w < RS_WARPS; ++w)
+      if (sBest[w].cost < b.cost) b = sBest[w];
+    best[(int64_t)pair * gridDim.x + blockIdx.x] = b;
+  }
+}
+
+// stage 2: every block's winner is locally optimised on its own, as in the essential path, then de-normalised to pixels:
+// F = T1^T Fn T0, unit Frobenius norm.  The record keeps its layout; its cost stays in the pair's normalised units, which all
+// blocks of the pair share, so the final launch compares like with like.
+// (One block per SM in the launch bound: under the default, ptxas caps the kernel at 128 registers and spills.)
+__global__ void __launch_bounds__(RS_THREADS, 1) ransac_f_lo_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
+                                                                 const int* __restrict__ np, int n_max, float thr,
+                                                                 RsRecord* __restrict__ best) {
+  extern __shared__ float4 sPts[];
+  __shared__ float red[4 * RS_WARPS];
+  __shared__ float sF[9];
+  const int pair = blockIdx.y;
+  const int n = min(np ? np[pair] : n_max, min(n_max, RS_MAX_PTS));
+  if (n < 8) return;
+  RsRecord* rec = best + (int64_t)pair * gridDim.x + blockIdx.x;
+  if (!(rec->cost < 3.0e38f)) return;                // this block found no hypothesis (block-uniform)
+  const RsPairNorm nz = rs_pair_normalise(p0 + (int64_t)pair * n_max * 2, p1 + (int64_t)pair * n_max * 2, n, sPts, red);
+  if (threadIdx.x < 9) sF[threadIdx.x] = rec->m[threadIdx.x];
+  const float cost = rs_f_local_opt(sPts, n, (thr * nz.s) * (thr * nz.s), sF);
+  if (threadIdx.x == 0) {
+    // T_i = [s 0 -s cx_i; 0 s -s cy_i; 0 0 1]:  F = T1^T Fn T0
+    const double s = nz.s, t0[2] = {-s * nz.cx0, -s * nz.cy0}, t1[2] = {-s * nz.cx1, -s * nz.cy1};
+    double A[9], F[9];                               // A = Fn T0
+    for (int r = 0; r < 3; ++r) {
+      const double f0 = sF[3 * r], f1 = sF[3 * r + 1], f2 = sF[3 * r + 2];
+      A[3 * r] = f0 * s; A[3 * r + 1] = f1 * s; A[3 * r + 2] = f0 * t0[0] + f1 * t0[1] + f2;
+    }
+    for (int c = 0; c < 3; ++c) {                    // F = T1^T A
+      F[c] = s * A[c]; F[3 + c] = s * A[3 + c]; F[6 + c] = t1[0] * A[c] + t1[1] * A[3 + c] + A[6 + c];
+    }
+    double nrm = 0.0;
+    for (int k = 0; k < 9; ++k) nrm += F[k] * F[k];
+    const double inv = nrm > 1e-300 ? 1.0 / sqrt(nrm) : 0.0;
+    for (int k = 0; k < 9; ++k) rec->m[k] = (float)(F[k] * inv);
+    rec->cost = cost;
+  }
+}
+
 }  // namespace xf
 
 extern "C" size_t xfeat_ransac_workspace_bytes(int batch, int iters) {
@@ -699,6 +980,31 @@ extern "C" int xfeat_ransac_essential(const float* d_x0, const float* d_x1, cons
   XF_LAUNCH_CHECK();
   xf::ransac_e_final_kernel<<<batch, xf::RS_THREADS, 0, st>>>(d_x0, d_x1, d_n, n_max, thr, (const xf::RsRecord*)d_ws, bpp, d_E,
                                                                  d_inliers, d_n_inliers);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" int xfeat_ransac_fundamental(const float* d_pts0, const float* d_pts1, const int32_t* d_n, const int32_t* d_pair_ids,
+                                        int n_max, int batch, float thr_px, int iters, uint32_t seed, float* d_F,
+                                        uint8_t* d_inliers, int32_t* d_n_inliers, void* d_ws, size_t ws_bytes, void* stream) {
+  XF_REQUIRE(d_pts0 && d_pts1 && d_F && d_inliers && d_n_inliers && d_ws, "ransac_fundamental: null pointer");
+  XF_REQUIRE(batch > 0 && batch <= 65535 && n_max > 0 && n_max <= xf::RS_MAX_PTS && iters > 0 && thr_px > 0.f,
+             "ransac_fundamental: bad arguments (n_max <= %d)", xf::RS_MAX_PTS);
+  XF_REQUIRE(ws_bytes >= xfeat_ransac_workspace_bytes(batch, iters), "ransac_fundamental: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int bpp = xf::cdiv(iters, xf::RS_WARPS * 32);          // one round = one 7-point sample per lane
+  const int rounds = xf::cdiv(iters, bpp * xf::RS_WARPS * 32);
+  const size_t smem = (size_t)n_max * sizeof(float4);
+  XF_DYN_SMEM(xf::ransac_f_hyp_kernel, smem);
+  XF_DYN_SMEM(xf::ransac_f_lo_kernel, smem);
+  xf::ransac_f_hyp_kernel<<<dim3(bpp, batch), xf::RS_THREADS, smem, st>>>(d_pts0, d_pts1, d_n, d_pair_ids, n_max, thr_px, rounds,
+                                                                          seed, (xf::RsRecord*)d_ws);
+  XF_LAUNCH_CHECK();
+  xf::ransac_f_lo_kernel<<<dim3(bpp, batch), xf::RS_THREADS, smem, st>>>(d_pts0, d_pts1, d_n, n_max, thr_px, (xf::RsRecord*)d_ws);
+  XF_LAUNCH_CHECK();
+  // the records now hold pixel F: the essential path's final launch classifies with `Sampson < thr_px` in pixels
+  xf::ransac_e_final_kernel<<<batch, xf::RS_THREADS, 0, st>>>(d_pts0, d_pts1, d_n, n_max, thr_px, (const xf::RsRecord*)d_ws, bpp,
+                                                                 d_F, d_inliers, d_n_inliers);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -89,6 +89,68 @@ def find_essential_batch(x0: torch.Tensor, x1: torch.Tensor, counts: Optional[to
     return E, mask.bool(), n_inl
 
 
+def find_fundamental_batch(pts0: torch.Tensor, pts1: torch.Tensor, counts: Optional[torch.Tensor] = None, thr: float = 3.0,
+                           iters: int = 2048, seed: int = 0, pair_ids=None,
+                           workspace: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Fundamental-matrix RANSAC for a batch of pairs: what cv2.findFundamentalMat(p0, p1, cv2.USAC_MAGSAC, thr) computes per
+    pair, for uncalibrated, non-planar pairs (photo collections, the 1500-pair benchmarks).  pts0, pts1: (B, n_max, 2) float32
+    CUDA tensors of matched PIXEL coordinates (pair b uses the first counts[b] rows; None: all; n_max <= 8192).
+    Returns F (B,3,3) float32 with x1^T F x0 = 0 in homogeneous pixels (unit Frobenius norm), inliers (B, n_max) bool and
+    n_inliers (B) int32 (a negative count passes through; fewer than 8 correspondences: zero F, no inliers).
+
+    `thr`: Sampson distance in pixels, the USAC meaning of cv2's ransacReprojThreshold (3.0 is cv2's default).  `iters`: 7-point
+    samples per pair; 2048 because an all-inlier sample has probability w^7, 6.4e-4 at w = 0.35, so 2048 samples draw about
+    1.3 of them, and the local optimisation recovers the full consensus set from a near-all-inlier one.  `pair_ids` (B ints,
+    default 0..B-1) seed each pair's samples: with its id fixed, a pair's result does not depend on its batch.  `workspace`: as
+    find_homography_batch.  A planar scene has no unique F: no degeneracy test is made."""
+    lib = _lib.load()
+    if not (pts0.is_cuda and pts1.is_cuda):
+        raise RuntimeError("find_fundamental_batch runs on the GPU only (no CPU fallback)")
+    p0 = pts0.float().contiguous()
+    p1 = pts1.float().contiguous()
+    if p0.ndim != 3 or p0.shape != p1.shape or p0.shape[-1] != 2:
+        raise RuntimeError("points must be two (B, n, 2) tensors of the same shape")
+    B, n_max, _ = p0.shape
+    dev = p0.device
+    F = torch.zeros((B, 3, 3), dtype=torch.float32, device=dev)
+    mask = torch.zeros((B, n_max), dtype=torch.uint8, device=dev)
+    n_inl = torch.zeros((B,), dtype=torch.int32, device=dev)
+    if B == 0 or n_max == 0:
+        return F, mask.bool(), n_inl
+    cnt = None if counts is None else counts.to(dev).to(torch.int32).contiguous()
+    ids = None
+    if pair_ids is not None:
+        ids = torch.as_tensor(pair_ids).to(device=dev, dtype=torch.int32).reshape(-1).contiguous()
+        if ids.numel() != B:
+            raise RuntimeError(f"pair_ids must hold one id per pair ({B}), got {ids.numel()}")
+    ws = workspace
+    if ws is None:
+        ws = torch.empty(max(256, lib.xfeat_ransac_workspace_bytes(B, iters)), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.xfeat_ransac_fundamental(p0.data_ptr(), p1.data_ptr(), None if cnt is None else cnt.data_ptr(),
+                                                None if ids is None else ids.data_ptr(), n_max, B, float(thr), int(iters),
+                                                int(seed) & 0xffffffff, F.data_ptr(), mask.data_ptr(), n_inl.data_ptr(),
+                                                ws.data_ptr(), ws.numel(), torch.cuda.current_stream(dev).cuda_stream),
+                   "xfeat_ransac_fundamental")
+    return F, mask.bool(), n_inl
+
+
+def find_fundamental(points1, points2, thr: float = 3.0, iters: int = 2048, seed: int = 0,
+                     device: Optional[torch.device] = None):
+    """cv2.findFundamentalMat-shaped call for ONE pair: (N,2) pixel arrays -> (F (3,3) float64 or None, mask (N,1) uint8).
+    None (and an empty mask) below 8 correspondences or 8 inliers.  Arguments as find_fundamental_batch."""
+    dev = device or torch.device("cuda", torch.cuda.current_device())
+    p0 = torch.as_tensor(np.asarray(points1, dtype=np.float32)).reshape(1, -1, 2).to(dev)
+    p1 = torch.as_tensor(np.asarray(points2, dtype=np.float32)).reshape(1, -1, 2).to(dev)
+    n = p0.shape[1]
+    if n < 8:
+        return None, np.zeros((n, 1), np.uint8)
+    F, mask, n_inl = find_fundamental_batch(p0, p1, None, thr, iters, seed)
+    if int(n_inl.item()) < 8:
+        return None, np.zeros((n, 1), np.uint8)
+    return F[0].double().cpu().numpy(), mask[0].to(torch.uint8).cpu().numpy().reshape(-1, 1)
+
+
 def recover_pose(E: np.ndarray, x0: np.ndarray, x1: np.ndarray):
     """(R, t) with X1 = R X0 + t from an essential matrix and normalised inlier correspondences: the candidate (of the four
     decompositions) that puts the most triangulated points in front of both cameras (what cv2.recoverPose does)."""

@@ -8,9 +8,10 @@ There is no CPU / eager fallback: without a CUDA device and the built library th
 Beyond the reference surface: `match_xfeat_batch` (batched match_xfeat) and `match_xfeat_stream` (pinned, double-buffered
 host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match_lighterglue_batch` and
 `match_xfeat_lighterglue_batch` (LighterGlue on batches of pairs, csrc/lighterglue.cu), `match_xfeat_pairs` and
-`match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once), and
+`match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once),
 `match_xfeat_star_pairs` (the same for semi-dense matching: XFeat* over a list of pairs, each image extracted once per scale),
-and `tracker` (one reference tracked through a video stream, each frame's step replayed as one CUDA graph; tracker.py).
+`tracker` (one reference tracked through a video stream, each frame's step replayed as one CUDA graph; tracker.py), and
+`match_xfeat_verified_pairs` (match_xfeat_pairs followed on the device by a fundamental-matrix RANSAC per pair; geometry.py).
 """
 from __future__ import annotations
 
@@ -861,9 +862,33 @@ class XFeat(torch.nn.Module):
         plan = PairPlan([pair_image_key(x) for x in images], pairs)
         if len(plan.pairs) == 0:
             return []
+        return self._pairs_matched(images, plan, top_k, min_cossim, "match_xfeat_pairs")
+
+    @torch.inference_mode()
+    def match_xfeat_verified_pairs(self, images, pairs, top_k=None, min_cossim=-1, ransac_thr: float = 3.0, iters: int = 2048,
+                                   seed: int = 0) -> List[Dict[str, np.ndarray]]:
+        """match_xfeat_pairs (same inputs, same extraction, same matches bit for bit) followed, still on the device, by the
+        fundamental-matrix RANSAC of geometry.find_fundamental_batch on every pair: the cv2.findFundamentalMat(mkpts0, mkpts1,
+        cv2.USAC_MAGSAC, ransac_thr) step that pair lists from photo collections run next.  Result p: {'mkpts0', 'mkpts1' (N,2),
+        'inliers' (N,) bool, 'n_inliers' int, 'F' (3,3) float64 with x1^T F x0 = 0 in pixels, or None when fewer than 8 inliers
+        support it}.  Pair p's samples are seeded by (seed, p), so its result is what find_fundamental_batch gives its matches
+        alone with pair_ids=[p].  One host synchronisation per chunk of pairs.  top_k above 8192 is refused."""
+        if top_k is None: top_k = self.top_k
+        if top_k > 8192:
+            raise ValueError(f"match_xfeat_verified_pairs: top_k {top_k} > 8192 (the RANSAC caches at most 8192 matches per pair)")
+        plan = PairPlan([pair_image_key(x) for x in images], pairs)
+        if len(plan.pairs) == 0:
+            return []
+        return self._pairs_matched(images, plan, top_k, min_cossim, "match_xfeat_verified_pairs", (ransac_thr, iters, seed))
+
+    def _pairs_matched(self, images, plan: PairPlan, top_k: int, min_cossim: float, what: str, ransac=None) -> List:
+        """The body of match_xfeat_pairs over a non-empty plan, and with `ransac` = (thr, iters, seed) that of
+        match_xfeat_verified_pairs: each chunk's matches go through find_fundamental_batch on the device before the chunk's one
+        host sync."""
         presplit = self._lib.xfeat_get_mnn_impl() in (1, 2, 3)   # else: fp32 descriptors, per-pair gather, xfeat_mnn_match_bounded
         order = plan.match_order()
         tp_all = torch.from_numpy(np.ascontiguousarray(plan.table_pairs[order])).to(self.dev)
+        ids_all = torch.from_numpy(order.astype(np.int32)).to(self.dev) if ransac else None    # match_order() reorders the pairs
         tab = self._extract_table(images, plan, top_k, want_split=presplit, want_desc=not presplit)
         out: List = [None] * len(order)
         step = PAIRS_MATCH_CHUNK if presplit else 256              # the fp32 fallback gathers (B, top_k, 64) per side
@@ -871,16 +896,26 @@ class XFeat(torch.nn.Module):
             sel, tp = order[o:o + step], tp_all[o:o + step]
             B = len(sel)
             mk0, mk1, cnt = self._match_table_pairs(tab, tp, top_k, min_cossim, presplit)
-            h0, h1 = (torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (mk0, mk1))
-            hc = torch.empty((B,), dtype=torch.int32, pin_memory=True)
-            for h, t in ((h0, mk0), (h1, mk1), (hc, cnt)):
+            dev_out = [mk0, mk1, cnt]
+            if ransac:
+                from .geometry import find_fundamental_batch
+                F, mask, n_inl = find_fundamental_batch(mk0, mk1, cnt, ransac[0], ransac[1], ransac[2], pair_ids=ids_all[o:o + step])
+                dev_out += [F, mask, n_inl]
+            host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in dev_out]
+            for h, t in zip(host, dev_out):
                 h.copy_(t, non_blocking=True)
             torch.cuda.current_stream(self.dev).synchronize()         # the only host sync of this chunk
-            c = hc.tolist()
-            self._check_counts(c, "match_xfeat_pairs", self._pair_labels(plan, sel))
-            a0, a1 = h0.numpy(), h1.numpy()
+            c = host[2].tolist()
+            self._check_counts(c, what, self._pair_labels(plan, sel))
+            a0, a1 = host[0].numpy(), host[1].numpy()
+            if not ransac:
+                for b, p in enumerate(sel.tolist()):
+                    out[p] = (a0[b, :c[b]].copy(), a1[b, :c[b]].copy())
+                continue
+            Fh, mh, nh = host[3].numpy(), host[4].numpy(), host[5].tolist()
             for b, p in enumerate(sel.tolist()):
-                out[p] = (a0[b, :c[b]].copy(), a1[b, :c[b]].copy())
+                out[p] = {"mkpts0": a0[b, :c[b]].copy(), "mkpts1": a1[b, :c[b]].copy(), "inliers": mh[b, :c[b]].copy(),
+                          "n_inliers": nh[b], "F": Fh[b].astype(np.float64) if nh[b] >= 8 else None}
         return out
 
     @torch.inference_mode()
