@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_h_final_kernel(const float*
   __shared__ float red[3 * RS_WARPS];
   __shared__ double sAcc[RS_WARPS][45];
   __shared__ float sH[9];
-  __shared__ int sCnt;
+  __shared__ int sCnt, sFound;
   const int pair = blockIdx.x;
   const int n_all = np ? np[pair] : n_max;
   const int n = min(n_all, min(n_max, RS_MAX_PTS));
@@ -265,8 +265,16 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_h_final_kernel(const float*
       if (c.cost < b.cost) b = c;
     }
     for (int k = 0; k < 9; ++k) sH[k] = b.m[k];
+    sFound = b.cost < 3.0e38f;
   }
   __syncthreads();
+  if (!sFound) {          // every 4-point sample was degenerate (identical or collinear points): no model, as for n < 4
+    if (threadIdx.x == 0) {
+      n_inl[pair] = 0;
+      for (int k = 0; k < 9; ++k) H_out[pair * 9 + k] = (k % 4 == 0) ? 1.f : 0.f;
+    }
+    return;
+  }
   const float t2 = (thr * n1.s) * (thr * n1.s);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int round = 0; round < 2; ++round) {

@@ -17,6 +17,9 @@ def find_homography_batch(pts0: torch.Tensor, pts1: torch.Tensor, counts: Option
                           workspace: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """pts0, pts1: (B, n_max, 2) float32 CUDA tensors of matched coordinates (pair b uses the first counts[b] rows; None: all).
     Returns H (B,3,3) float32 with H[2,2] = 1 mapping image-0 to image-1 pixels, inliers (B, n_max) bool, n_inliers (B) int32.
+    A pair with fewer than 4 correspondences, or whose every 4-point sample is degenerate (all points identical, all exactly
+    on one line, fewer than 4 distinct points), has no model: identity H, no inliers, n_inliers 0 (a negative count passes
+    through).
     `thr`: forward transfer error in pixels of image 1 (cv2's ransacReprojThreshold).  `workspace`: a uint8 CUDA tensor of at
     least xfeat_ransac_workspace_bytes(B, iters) bytes to use as scratch (default: a fresh one), for callers that capture the
     call into a CUDA graph and keep the scratch alive with it."""
