@@ -62,6 +62,7 @@ SIGNATURES = {
     "xfeat_ransac_homography": (c_i, [c_p, c_p, c_p, c_i, c_i, c_f, c_i, C.c_uint32, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_ransac_essential": (c_i, [c_p, c_p, c_p, c_i, c_i, c_f, c_i, C.c_uint32, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_ransac_fundamental": (c_i, [c_p, c_p, c_p, c_p, c_i, c_i, c_f, c_i, C.c_uint32, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_debug_seven_point": (c_i, [c_p, c_i, c_p, c_p, c_p]),
     "xfeat_lg_packed_weight_floats": (c_sz, []),
     "xfeat_lg_create": (c_i, [C.POINTER(c_p), c_i, c_p, c_sz]),
     "xfeat_lg_destroy": (None, [c_p]),

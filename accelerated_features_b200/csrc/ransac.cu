@@ -703,8 +703,8 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_e_final_kernel(const float*
 // ---------------------------------------------------------------------------------------------------------------------
 // Fundamental matrix (uncalibrated two-view geometry; what cv2.findFundamentalMat(p0, p1, cv2.USAC_*, thr) computes).  Inputs
 // are PIXELS.  Every lane solves one 7-point sample in fp64 (1-3 candidates), the warp scores them with MSAC on the Sampson
-// distance, every block's winner is locally optimised (rs_f_local_opt), and the essential path's final launch classifies
-// with the de-normalised pixel F.  thr is the USAC meaning: Sampson distance in pixels (OpenCV 4.13's USAC_DEFAULT /
+// distance, every block's winner is locally optimised (rs_f_local_opt), and ransac_f_final_kernel classifies with the
+// de-normalised pixel F, in fp64.  thr is the USAC meaning: Sampson distance in pixels (OpenCV 4.13's USAC_DEFAULT /
 // USAC_ACCURATE / USAC_MAGSAC masks are exactly `Sampson < thr`).
 // ---------------------------------------------------------------------------------------------------------------------
 
@@ -810,6 +810,35 @@ __device__ int rs_seven_point(const double (&F1)[9], const double (&F2)[9], floa
   return nc;
 }
 
+// One 7-point sample, the body of a ransac_f_hyp_kernel lane: the 9 x 9 normal matrix of the seven epipolar rows of
+// pts[idx[0..6]] (normalised (x, y, u, v)), its two smallest eigenvectors (cyclic Jacobi) as the null space, and the 1-3
+// candidates of rs_seven_point.  Also run on its own by xfeat_debug_seven_point.
+__device__ __forceinline__ int rs_f_sample(const float4* pts, const int (&idx)[7], float (&Fc)[3][9]) {
+  double M[9][9];
+  for (int a = 0; a < 9; ++a)
+    for (int b2 = 0; b2 < 9; ++b2) M[a][b2] = 0.0;
+  for (int k = 0; k < 7; ++k) {
+    const float4 c = pts[idx[k]];
+    double r[9];
+    rs_epi_row(c.x, c.y, c.z, c.w, r);
+    for (int a = 0; a < 9; ++a)
+      for (int b2 = a; b2 < 9; ++b2) M[a][b2] += r[a] * r[b2];
+  }
+  for (int a = 0; a < 9; ++a)
+    for (int b2 = 0; b2 < a; ++b2) M[a][b2] = M[b2][a];
+  double V[9][9];
+  rs_jacobi<9>(M, V);
+  int i1 = 0, i2 = 1;                           // the two smallest eigenvalues: the null space of the 7 x 9 system
+  if (M[i2][i2] < M[i1][i1]) { i1 = 1; i2 = 0; }
+  for (int i = 2; i < 9; ++i) {
+    if (M[i][i] < M[i1][i1]) { i2 = i1; i1 = i; }
+    else if (M[i][i] < M[i2][i2]) i2 = i;
+  }
+  double F1[9], F2[9];
+  for (int k = 0; k < 9; ++k) { F1[k] = V[k][i1]; F2[k] = V[k][i2]; }
+  return rs_seven_point(F1, F2, Fc);
+}
+
 // stage 1: grid (blocks_per_pair, batch).  Samples come from a hash of (seed, pair id, hypothesis id): with the id fixed, a
 // pair's result does not depend on the batch it is in.
 __global__ void __launch_bounds__(RS_THREADS) ransac_f_hyp_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
@@ -844,30 +873,8 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_f_hyp_kernel(const float* _
           for (int j = 0; j < k; ++j) dup |= (idx[j] == idx[k]);
         } while (dup);
       }
-      double M[9][9];
-      for (int a = 0; a < 9; ++a)
-        for (int b2 = 0; b2 < 9; ++b2) M[a][b2] = 0.0;
-      for (int k = 0; k < 7; ++k) {
-        const float4 c = sPts[idx[k]];
-        double r[9];
-        rs_epi_row(c.x, c.y, c.z, c.w, r);
-        for (int a = 0; a < 9; ++a)
-          for (int b2 = a; b2 < 9; ++b2) M[a][b2] += r[a] * r[b2];
-      }
-      for (int a = 0; a < 9; ++a)
-        for (int b2 = 0; b2 < a; ++b2) M[a][b2] = M[b2][a];
-      double V[9][9];
-      rs_jacobi<9>(M, V);
-      int i1 = 0, i2 = 1;                           // the two smallest eigenvalues: the null space of the 7 x 9 system
-      if (M[i2][i2] < M[i1][i1]) { i1 = 1; i2 = 0; }
-      for (int i = 2; i < 9; ++i) {
-        if (M[i][i] < M[i1][i1]) { i2 = i1; i1 = i; }
-        else if (M[i][i] < M[i2][i2]) i2 = i;
-      }
-      double F1[9], F2[9];
-      for (int k = 0; k < 9; ++k) { F1[k] = V[k][i1]; F2[k] = V[k][i2]; }
       float Fc[3][9];
-      const int nc = rs_seven_point(F1, F2, Fc);
+      const int nc = rs_f_sample(sPts, idx, Fc);
       // the warp scores the lanes' candidates (up to 96) one after the other
       for (int src = 0; src < 32; ++src) {
         const int ncs = __shfl_sync(0xffffffffu, nc, src);
@@ -937,6 +944,83 @@ __global__ void __launch_bounds__(RS_THREADS, 1) ransac_f_lo_kernel(const float*
     for (int k = 0; k < 9; ++k) rec->m[k] = (float)(F[k] * inv);
     rec->cost = cost;
   }
+}
+
+// Squared Sampson distance in pixels under the float32 pixel F, evaluated in fp64.  Far from the origin x1^T F x0 is the
+// cancellation of terms many orders larger than itself: at coordinates near (7000, 5000), rs_sampson2's float32 evaluation is
+// off by up to 0.17 px, so the mask would not be `Sampson < thr` under the returned F.
+__device__ __forceinline__ double rs_sampson2_px(const float (&F)[9], double x, double y, double u, double v) {
+  const double a = F[0] * x + F[1] * y + F[2], b = F[3] * x + F[4] * y + F[5], c = F[6] * x + F[7] * y + F[8];
+  const double d = F[0] * u + F[3] * v + F[6], f = F[1] * u + F[4] * v + F[7];
+  const double e = u * a + v * b + c;
+  const double den = a * a + b * b + d * d + f * f;
+  return den > 1e-300 ? e * e / den : 1e300;
+}
+
+// stage 3: the best optimised candidate classifies the correspondences: inlier iff its pixel Sampson distance under the returned
+// F is below thr, in fp64.
+__global__ void __launch_bounds__(RS_THREADS) ransac_f_final_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
+                                                                    const int* __restrict__ np, int n_max, float thr,
+                                                                    const RsRecord* __restrict__ best, int blocks_per_pair,
+                                                                    float* __restrict__ F_out, unsigned char* __restrict__ mask,
+                                                                    int* __restrict__ n_inl) {
+  __shared__ float sF[9];
+  __shared__ int sCnt;
+  const int pair = blockIdx.x;
+  const int n_all = np ? np[pair] : n_max;
+  const int n = min(n_all, min(n_max, RS_MAX_PTS));
+  unsigned char* mk = mask + (int64_t)pair * n_max;
+  for (int i = threadIdx.x; i < n_max; i += RS_THREADS) mk[i] = 0;
+  if (n < 8) {
+    if (threadIdx.x == 0) {
+      n_inl[pair] = n_all < 0 ? n_all : 0;
+      for (int k = 0; k < 9; ++k) F_out[pair * 9 + k] = 0.f;
+    }
+    return;
+  }
+  const float* q0 = p0 + (int64_t)pair * n_max * 2;
+  const float* q1 = p1 + (int64_t)pair * n_max * 2;
+  if (threadIdx.x == 0) {
+    RsRecord b = best[(int64_t)pair * blocks_per_pair];
+    for (int k = 1; k < blocks_per_pair; ++k) {
+      const RsRecord c = best[(int64_t)pair * blocks_per_pair + k];
+      if (c.cost < b.cost) b = c;
+    }
+    for (int k = 0; k < 9; ++k) sF[k] = b.m[k];
+    sCnt = 0;
+  }
+  __syncthreads();
+  const double t2 = (double)thr * (double)thr;
+  const int lane = threadIdx.x & 31;
+  float F[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) F[k] = sF[k];
+  int cnt = 0;
+  for (int i = threadIdx.x; i < n; i += RS_THREADS) {
+    const bool in = rs_sampson2_px(F, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1]) < t2;
+    mk[i] = in ? 1 : 0;
+    cnt += in ? 1 : 0;
+  }
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) atomicAdd(&sCnt, cnt);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    n_inl[pair] = sCnt;
+    for (int k = 0; k < 9; ++k) F_out[pair * 9 + k] = F[k];
+  }
+}
+
+// Test hook: one thread per 7-point sample (7 normalised (x, y, u, v) rows), candidates zero-padded to 3.
+__global__ void __launch_bounds__(RS_THREADS) ransac_f_debug_seven_point_kernel(const float4* __restrict__ samples, int n_samples,
+                                                                                float* __restrict__ F_out, int* __restrict__ count) {
+  const int i = blockIdx.x * RS_THREADS + threadIdx.x;
+  if (i >= n_samples) return;
+  const int idx[7] = {0, 1, 2, 3, 4, 5, 6};
+  float Fc[3][9];
+  const int nc = rs_f_sample(samples + (int64_t)i * 7, idx, Fc);
+  for (int j = 0; j < 3; ++j)
+    for (int k = 0; k < 9; ++k) F_out[((int64_t)i * 3 + j) * 9 + k] = j < nc ? Fc[j][k] : 0.f;
+  count[i] = nc;
 }
 
 }  // namespace xf
@@ -1010,9 +1094,18 @@ extern "C" int xfeat_ransac_fundamental(const float* d_pts0, const float* d_pts1
   XF_LAUNCH_CHECK();
   xf::ransac_f_lo_kernel<<<dim3(bpp, batch), xf::RS_THREADS, smem, st>>>(d_pts0, d_pts1, d_n, n_max, thr_px, (xf::RsRecord*)d_ws);
   XF_LAUNCH_CHECK();
-  // the records now hold pixel F: the essential path's final launch classifies with `Sampson < thr_px` in pixels
-  xf::ransac_e_final_kernel<<<batch, xf::RS_THREADS, 0, st>>>(d_pts0, d_pts1, d_n, n_max, thr_px, (const xf::RsRecord*)d_ws, bpp,
+  // the records now hold pixel F: the final launch classifies with `Sampson < thr_px` in pixels
+  xf::ransac_f_final_kernel<<<batch, xf::RS_THREADS, 0, st>>>(d_pts0, d_pts1, d_n, n_max, thr_px, (const xf::RsRecord*)d_ws, bpp,
                                                                  d_F, d_inliers, d_n_inliers);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" int xfeat_debug_seven_point(const float* d_samples, int n_samples, float* d_F, int32_t* d_count, void* stream) {
+  XF_REQUIRE(d_samples && d_F && d_count, "debug_seven_point: null pointer");
+  XF_REQUIRE(n_samples > 0 && ((uintptr_t)d_samples & 15) == 0, "debug_seven_point: bad arguments (16-byte aligned samples)");
+  xf::ransac_f_debug_seven_point_kernel<<<xf::cdiv(n_samples, xf::RS_THREADS), xf::RS_THREADS, 0, (cudaStream_t)stream>>>(
+      (const float4*)d_samples, n_samples, d_F, d_count);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

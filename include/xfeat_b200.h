@@ -312,7 +312,7 @@ XF_API int xfeat_ransac_essential(const float* d_x0, const float* d_x1, const in
  * (batch) counts (NULL: n_max each).  Each pair is normalised with its two centroids and one shared scale; `iters` 7-point
  * samples (1-3 candidates each) are scored with MSAC on the Sampson distance, every block's winner is locally optimised
  * (Sampson-weighted 8-point refits projected to rank 2) and the best one classifies: inlier iff Sampson distance < thr_px, in
- * pixels (OpenCV's USAC meaning).  Outputs d_F (batch, 9) row-major, unit Frobenius norm, x1^T F x0 = 0 in homogeneous pixels;
+ * pixels (OpenCV's USAC meaning), evaluated in fp64 under the returned F.  Outputs d_F (batch, 9) row-major, unit Frobenius norm, x1^T F x0 = 0 in homogeneous pixels;
  * d_inliers (batch, n_max) 0/1; d_n_inliers (batch), a negative count (XF_N_OVERFLOW) passed through.  Fewer than 8 matches:
  * zero matrix, no inliers.  Samples are drawn from (seed, d_pair_ids[b]) (NULL: b), so with the ids fixed a pair's result does
  * not depend on its batch.  n_max <= 8192.  Planar scenes have no unique F (no degeneracy handling).  Workspace:
@@ -320,6 +320,11 @@ XF_API int xfeat_ransac_essential(const float* d_x0, const float* d_x1, const in
 XF_API int xfeat_ransac_fundamental(const float* d_pts0, const float* d_pts1, const int32_t* d_n, const int32_t* d_pair_ids,
                                     int n_max, int batch, float thr_px, int iters, uint32_t seed, float* d_F, uint8_t* d_inliers,
                                     int32_t* d_n_inliers, void* d_ws, size_t ws_bytes, void* stream);
+
+/* Test hook: the 7-point step of xfeat_ransac_fundamental alone, one sample per thread.  d_samples (n_samples, 7, 4) fp32 rows
+ * (x, y, u, v) in the pair's normalised frame, 16-byte aligned.  Outputs d_F (n_samples, 3, 9) row-major candidates with
+ * x1^T F x0 = 0, unit Frobenius norm, zero past the count; d_count (n_samples) int32, 0-3 (0: degenerate sample). */
+XF_API int xfeat_debug_seven_point(const float* d_samples, int n_samples, float* d_F, int32_t* d_count, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * LighterGlue matcher (csrc/lighterglue.cu; fp32 CUDA-core kernels), its own handle and weight blob

@@ -144,3 +144,122 @@ def test_recover_pose_exact_all_chirality_configurations():
             ti = 0 if np.abs(U[:, 2] - t).max() < 1e-9 else 1
             slots.add((ri, ti))
     assert slots == {(0, 0), (0, 1), (1, 0), (1, 1)}, slots
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# fundamental matrix
+# ---------------------------------------------------------------------------------------------------------------------------
+# (K0, size0, K1, size1): two cameras with different intrinsics and image sizes, and one shared
+F_CAMS = [(ref.intrinsics(700, 330, 235), (640, 480), ref.intrinsics(3000, 1900, 1100), (3840, 2160)),
+          (ref.intrinsics(60, 31, 25), (64, 48), ref.intrinsics(2500, 1950, 1070), (3840, 2160)),
+          (ref.intrinsics(560, 320, 240), (640, 480), ref.intrinsics(560, 320, 240), (640, 480))]
+
+
+def f_scene(rng, cam, n):
+    K0, s0, K1, s1 = cam
+    R, t = ref.rodrigues(rng.normal(0, 0.1, 3)), rng.normal(0, 0.5, 3)
+    p0, p1 = ref.two_view_points(rng, K0, K1, s0, s1, R, t, n)
+    return p0, p1, ref.fundamental_from_cameras(K0, K1, R, t)
+
+
+def sign_dist(A, B):
+    A, B = A / np.linalg.norm(A), B / np.linalg.norm(B)
+    return min(np.abs(A - B).max(), np.abs(A + B).max())
+
+
+def test_pair_normaliser_and_sampson_scale():
+    """The DESIGN claim behind the pixel threshold: with one scale s for both images, the Sampson distance of the normalised
+    points under Fn = T1^-T F T0^-1 is exactly s times the pixel one (to float64 rounding), however different the images."""
+    rng = np.random.default_rng(6)
+    for cam in F_CAMS:
+        p0, p1, F = f_scene(rng, cam, 300)
+        p1 = p1 + rng.normal(0, 2.0, p1.shape)                   # non-zero distances
+        cx0, cy0, cx1, cy1, s = nz = ref.pair_normaliser(p0, p1)
+        a, b = (p0 - [cx0, cy0]) * s, (p1 - [cx1, cy1]) * s
+        assert np.abs(a.mean(0)).max() < 1e-12 and np.abs(b.mean(0)).max() < 1e-12
+        md = np.concatenate([np.linalg.norm(a, axis=1), np.linalg.norm(b, axis=1)]).mean()
+        assert abs(md - np.sqrt(2)) < 1e-12
+        T0, T1 = ref.pair_norm_matrices(nz)
+        Fn = np.linalg.inv(T1).T @ F @ np.linalg.inv(T0)
+        d_px, d_n = ref.sampson(F, p0, p1), ref.sampson(Fn, a, b)
+        assert np.abs(d_n / (s * d_px) - 1).max() < 1e-9
+        assert np.allclose(T1.T @ Fn @ T0, F, rtol=0, atol=1e-12)
+    assert ref.pair_normaliser(np.full((9, 2), 5.0), np.full((9, 2), 7.0)) == (5.0, 5.0, 7.0, 7.0, 1.0)
+
+
+def test_det_cubic_matches_determinant():
+    rng = np.random.default_rng(8)
+    for _ in range(20):
+        A, B = rng.normal(size=(3, 3)), rng.normal(size=(3, 3))
+        c = ref.det_cubic(A, B)
+        for lam in (-2.0, -0.3, 0.0, 0.7, 3.0):
+            assert abs(np.polyval(c, lam) - np.linalg.det(A + lam * B)) < 1e-12 * (1 + abs(lam)) ** 3 * 30
+
+
+def test_seven_point_exact():
+    """On 7 exact correspondences of a non-planar scene, +-F_true is among the candidates; every candidate satisfies the 7
+    epipolar constraints, has unit norm and det = 0.  Both the one-root and the three-root case occur."""
+    rng = np.random.default_rng(9)
+    counts = set()
+    for k in range(60):
+        p0, p1, F = f_scene(rng, F_CAMS[k % len(F_CAMS)], 7)
+        T0, T1 = ref.pair_norm_matrices(ref.pair_normaliser(p0, p1))
+        a, b = (ref._h(p0) @ T0.T)[:, :2], (ref._h(p1) @ T1.T)[:, :2]
+        Fn_true = np.linalg.inv(T1).T @ F @ np.linalg.inv(T0)
+        cands, _ = ref.seven_point(a, b)
+        counts.add(len(cands))
+        assert 1 <= len(cands) <= 3
+        assert min(sign_dist(c, Fn_true) for c in cands) < 1e-8, k
+        for c in cands:
+            assert abs(np.linalg.norm(c) - 1) < 1e-12
+            assert np.abs(ref.epipolar_rows(a, b) @ c.ravel()).max() < 1e-12
+            assert abs(np.linalg.det(c)) < 1e-12
+    assert counts >= {1, 3}, counts
+
+
+def test_seven_point_root_at_infinity():
+    """When the basis makes det(F1 - F2) = 0, the cubic loses its leading term and F1 - F2 is itself a solution: it is returned
+    beside the roots of the remaining quadratic, each singular and in the span."""
+    rng = np.random.default_rng(10)
+    for _ in range(10):
+        Fa = ref.project_rank2(rng.normal(size=(3, 3)))
+        F2 = rng.normal(size=(3, 3))
+        cands, c = ref.seven_point_from_basis(F2 + Fa, F2)
+        assert abs(c[0]) < 1e-12 * np.abs(c).max()
+        assert sign_dist(cands[-1], Fa) < 1e-12
+        for G in cands:
+            assert abs(np.linalg.det(G)) < 1e-10
+            r = np.linalg.lstsq(np.stack([Fa.ravel(), F2.ravel()], 1), G.ravel(), rcond=None)[1]
+            assert r.size == 0 or r[0] < 1e-20
+
+
+def test_project_rank2_is_nearest():
+    rng = np.random.default_rng(11)
+    for _ in range(20):
+        M = rng.normal(size=(3, 3))
+        P = ref.project_rank2(M)
+        s = np.linalg.svd(M, compute_uv=False)
+        assert np.linalg.matrix_rank(P, tol=1e-10) == 2 and np.abs(ref.project_rank2(P) - P).max() < 1e-12
+        assert abs(np.linalg.norm(M - P) - s[2]) < 1e-12            # Eckart-Young: the distance is the dropped value
+        for _ in range(50):                                          # no random rank-2 matrix near M is nearer
+            Q = ref.project_rank2(P + rng.normal(0, 0.05, (3, 3)))
+            assert np.linalg.norm(M - Q) >= s[2] - 1e-12
+
+
+def test_f_lo_refit_exact():
+    """On exact inliers among far outliers, one refit from a slightly wrong F returns F_true (up to sign), whichever cameras."""
+    rng = np.random.default_rng(12)
+    for cam in F_CAMS:
+        p0, p1, F = f_scene(rng, cam, 400)
+        out = rng.uniform(size=400) < 0.4
+        W1, H1 = cam[3]
+        while True:
+            bad = out & (ref.sampson(F, p0, p1) < 30)
+            if not bad.any():
+                break
+            p1[bad] = rng.uniform([0, 0], [W1, H1], (bad.sum(), 2))
+        Fp = F + rng.normal(0, 1e-6, (3, 3)) * np.abs(F)
+        assert ref.sampson(Fp, p0[~out], p1[~out]).max() < 1.0
+        Fr = ref.f_lo_refit(Fp, p0, p1, 3.0)
+        assert sign_dist(Fr, F) < 1e-9 and abs(np.linalg.det(Fr)) < 1e-12
+        assert ref.sampson(Fr, p0[~out], p1[~out]).max() < 1e-8
