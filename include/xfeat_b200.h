@@ -300,7 +300,8 @@ XF_API int xfeat_ransac_homography(const float* d_pts0, const float* d_pts1, con
 /* replaces: the relative-pose RANSAC the 1500-pair benchmarks run on the matches (poselib.estimate_relative_pose,
  * modules/eval/megadepth1500.py:98-113): essential matrix from NORMALISED image coordinates d_x0 / d_x1 (batch, n_max, 2)
  * (K^-1 applied by the caller), 8-point hypotheses projected onto the essential manifold, Sampson distance against `thr` (in
- * normalised units: pixels / focal length), MSAC scoring, two least-squares re-fits.  Outputs d_E (batch, 9) row-major with
+ * normalised units: pixels / focal length), MSAC scoring, every block's winner locally optimised (8 Sampson-weighted 8-point
+ * refits projected onto the essential manifold), the best one classifies.  Outputs d_E (batch, 9) row-major with
  * x1^T E x0 = 0, d_inliers, d_n_inliers.  Fewer than 8 matches: zero matrix.  (The 8-point solver is degenerate for planar
  * scenes, unlike poselib's 5-point solver.)  Workspace: xfeat_ransac_workspace_bytes. */
 XF_API int xfeat_ransac_essential(const float* d_x0, const float* d_x1, const int32_t* d_n, int n_max, int batch, float thr,

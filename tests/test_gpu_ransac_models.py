@@ -258,8 +258,9 @@ def h_degenerate_scenes(rng):
 
 
 def test_homography_degenerate_inputs():
-    """Pairs with no non-degenerate 4-point sample report no model, like n < 4: identity H, empty mask, n_inliers 0, and
-    find_homography returns None.  A generic 4-point pair still gives its exact H; a negative count passes through."""
+    """Pairs with no non-degenerate 4-point sample report no model, like n < 4 and a batch with n_max = 0: identity H, empty
+    mask, n_inliers 0, and find_homography returns None.  A generic 4-point pair still gives its exact H; a negative count
+    passes through."""
     rng = np.random.default_rng(13)
     degen = h_degenerate_scenes(rng)
     Ht = motion_h("perspective", 640, 480)
@@ -282,6 +283,9 @@ def test_homography_degenerate_inputs():
     assert np.array_equal(mask[b + 1, :300], good[2]) and n_inl[b + 1] == good[2].sum()
     for b, want in ((len(scenes) - 2, 0), (len(scenes) - 1, _lib.N_OVERFLOW)):
         assert np.array_equal(Hg[b], np.eye(3, dtype=F32)) and not mask[b].any() and n_inl[b] == want
+    # a batch without correspondences (n_max = 0): every pair has no model
+    Hg, mask, n_inl = run_h(np.zeros((3, 0, 2), F32), np.zeros((3, 0, 2), F32), None, H_THR, 1024, seed=2)
+    assert np.array_equal(Hg, np.broadcast_to(np.eye(3, dtype=F32), (3, 3, 3))) and mask.shape == (3, 0) and not n_inl.any()
 
 
 def test_homography_deterministic_and_isolated():
@@ -684,7 +688,7 @@ def cubic_scan(rng, m):
 
 
 def test_seven_point_solver_vs_float64():
-    """The 7-point step of ransac_f_hyp_kernel (normal matrix, Jacobi null space, cubic, roots, Newton polish) through
+    """The 7-point step of ransac_hyp_kernel<RsFundamental> (normal matrix, Jacobi null space, cubic, roots, Newton polish) through
     xfeat_debug_seven_point, against seven_point in float64 on the same float32 samples.  The candidate set does not depend on
     the null-space basis, so sets are compared up to sign: equal counts and each candidate close to one of the other side's.
     Where the cubic is close to losing a root (cubic_flags) a count difference is allowed and reported; every GPU candidate
@@ -835,7 +839,7 @@ def test_fundamental_mask_is_sampson_below_thr(thr):
     """The mask is `Sampson < thr` under the returned F, in float64 from the pixel points, on the three sizes, the mixed pairs
     and a pair near (7000, 5000); n_inliers is its size, nothing is set past the count, F is unit norm and rank 2.  Near
     (7000, 5000) a float32 evaluation of the pixel Sampson distance is off by up to 0.17 px, which fails this at 0.5 px: the
-    classification is made in fp64 (ransac_f_final_kernel)."""
+    classification is made in fp64 (ransac_final_kernel<RsFundamental>)."""
     rng = np.random.default_rng(int(thr * 10) + 90)
     keys, scenes = [], []
     for pair in SAME_PAIRS + MIXED_PAIRS:
