@@ -168,6 +168,8 @@ extern int g_conv_impl;  // 0 = fp32 CUDA cores, 1 = wgmma (per-tap operand load
 bool conv_tc_eligible(int layer);
 int launch_conv_tc_halo(const xfeat_ctx* ctx, int layer, const __half* in_split, int B, int H, int W, __half* out_split,
                         float* out_f32, cudaStream_t st);
+int launch_stem_tail_halo(const xfeat_ctx* ctx, const __half* a2_split, const float* xn, int B, int H2, int W2, __half* out_split,
+                          cudaStream_t st);
 int launch_topk_select_sort(const unsigned long long* keys, const int* n_keep, int n_const, int cap, int top_k, int B,
                             unsigned long long* sorted, cudaStream_t st);
 int conv_tc_prepare(xfeat_ctx* ctx);

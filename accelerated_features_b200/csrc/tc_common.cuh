@@ -309,16 +309,55 @@ __device__ __forceinline__ void conv_store_piece(unsigned char* stg, uint32_t& p
   ++piece;
 }
 
-// Bias, ReLU, block1.3's skip term, then the split x = hi + lo -- per value in the order the model defines.  srow[h] is the
-// staging row of fragment row h (r, r+8, r+64, r+72), or -1 for a GEMM row that is no output pixel (halo junk lanes).
+// Channels per epilogue block (CB) and 8-column fragment groups per block (JB).
+template <int NOUT>
+struct EpiBlock {
+  static constexpr int CB = NOUT < 32 ? NOUT : 32;
+  static constexpr int JB = CB / 8;
+};
+
+// The values of channel block cb: bias, ReLU, block1.3's skip term (sv[h], the pooled input of fragment row h), then the split
+// x = hi + lo -- per value in the order the model defines.  Thread q = lane % 4 gets channels 8j + 2q + e of fragment rows
+// r, r+8, r+64, r+72 as o[h][jj][e], and the packed half2 pairs hi[h][jj], lo[h][jj].
+template <int NOUT>
+__device__ __forceinline__ void conv_values(const float (&d0)[NOUT], const float (&d1)[NOUT], int cb, const float (&sv)[4],
+                                            const ConvEpi& E, float (&o)[4][EpiBlock<NOUT>::JB][2],
+                                            uint32_t (&hi)[4][EpiBlock<NOUT>::JB], uint32_t (&lo)[4][EpiBlock<NOUT>::JB]) {
+  constexpr int JB = EpiBlock<NOUT>::JB;
+  constexpr int G1 = NOUT / 8;                // fragment group of the group-1 column of channel 0
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+#pragma unroll
+    for (int jj = 0; jj < JB; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = cb * JB + jj, c = 8 * j + 2 * q + e, i = 2 * (h & 1) + e;
+        const float g0 = (h < 2) ? d0[4 * j + i] : d1[4 * j + i];
+        const float g1 = (h < 2) ? d0[4 * (j + G1) + i] : d1[4 * (j + G1) + i];
+        float t = fmaf(g0 + g1, E.inv_wscale, E.bias[c]);
+        if (E.relu) t = fmaxf(t, 0.f);
+        if (E.skip_w != nullptr) t += fmaf(sv[h], E.skip_w[c], E.skip_w[NOUT + c]);
+        o[h][jj][e] = t;
+      }
+      const __half2 hh = __floats2half2_rn(o[h][jj][0], o[h][jj][1]);
+      const float2 hf = __half22float2(hh);
+      const __half2 ll = __floats2half2_rn(o[h][jj][0] - hf.x, o[h][jj][1] - hf.y);
+      hi[h][jj] = *reinterpret_cast<const uint32_t*>(&hh);
+      lo[h][jj] = *reinterpret_cast<const uint32_t*>(&ll);
+    }
+  }
+}
+
+// conv_values, then the TMA stores.  srow[h] is the staging row of fragment row h (r, r+8, r+64, r+72), or -1 for a GEMM row
+// that is no output pixel (halo junk lanes).
 template <int NOUT>
 __device__ __forceinline__ void conv_epilogue(const float (&d0)[NOUT], const float (&d1)[NOUT], unsigned char* stg, uint32_t& piece,
                                               const int (&srow)[4], const ConvEpi& E) {
   static_assert(NOUT == 8 || NOUT == 32 || NOUT == 64, "conv_epilogue: NOUT");
-  constexpr int CB = NOUT < 32 ? NOUT : 32;   // channels per block
-  constexpr int JB = CB / 8;                  // 8-column fragment groups per block
+  constexpr int CB = EpiBlock<NOUT>::CB;      // channels per block
+  constexpr int JB = EpiBlock<NOUT>::JB;      // 8-column fragment groups per block
   constexpr int RB = NOUT < 32 ? 32 : 64;     // staging row bytes
-  constexpr int G1 = NOUT / 8;                // fragment group of the group-1 column of channel 0
   const int q = threadIdx.x & 3;
   float sv[4];
 #pragma unroll
@@ -327,27 +366,7 @@ __device__ __forceinline__ void conv_epilogue(const float (&d0)[NOUT], const flo
   for (int cb = 0; cb < NOUT / CB; ++cb) {
     float o[4][JB][2];
     uint32_t hi[4][JB], lo[4][JB];
-#pragma unroll
-    for (int h = 0; h < 4; ++h) {
-#pragma unroll
-      for (int jj = 0; jj < JB; ++jj) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int j = cb * JB + jj, c = 8 * j + 2 * q + e, i = 2 * (h & 1) + e;
-          const float g0 = (h < 2) ? d0[4 * j + i] : d1[4 * j + i];
-          const float g1 = (h < 2) ? d0[4 * (j + G1) + i] : d1[4 * (j + G1) + i];
-          float t = fmaf(g0 + g1, E.inv_wscale, E.bias[c]);
-          if (E.relu) t = fmaxf(t, 0.f);
-          if (E.skip_w != nullptr) t += fmaf(sv[h], E.skip_w[c], E.skip_w[NOUT + c]);
-          o[h][jj][e] = t;
-        }
-        const __half2 hh = __floats2half2_rn(o[h][jj][0], o[h][jj][1]);
-        const float2 hf = __half22float2(hh);
-        const __half2 ll = __floats2half2_rn(o[h][jj][0] - hf.x, o[h][jj][1] - hf.y);
-        hi[h][jj] = *reinterpret_cast<const uint32_t*>(&hh);
-        lo[h][jj] = *reinterpret_cast<const uint32_t*>(&ll);
-      }
-    }
+    conv_values<NOUT>(d0, d1, cb, sv, E, o, hi, lo);
     if (E.split != nullptr) {
       if constexpr (NOUT == 8) {   // one piece of whole [hi(8) | lo(8)] rows
         conv_store_piece(stg, piece, E.split, 0, E, [&](unsigned char* buf) {

@@ -383,6 +383,12 @@ XF_API int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* 
                                         void* d_out_split, const float* d_skip_xn, void* d_scratch, size_t scratch_bytes,
                                         void* stream);
 
+/* Test hook: the stem tail xfeat_net runs (block1.2, then block1.3 + skip1, in one kernel).  d_in (B,H2,W2,8) fp32 NHWC is
+ * block1.1's output, split into d_scratch (>= B*H2*W2*32 bytes) as xfeat_debug_conv_layer_tc_ex splits it; d_xn the normalised
+ * gray image (B,2*H2,2*W2) fp32; d_out_split (B,H2/2,W2/2,64) fp16 [hi(32) | lo(32)], channels 24-31 zero.  H2, W2 even. */
+XF_API int xfeat_debug_stem_tail(xfeat_ctx* ctx, const float* d_in, const float* d_xn, int B, int H2, int W2, void* d_out_split,
+                                 void* d_scratch, size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,7 +11,8 @@ OUT/kernels.json, and prints the card's name, power limit and maximum SM clock.
 
 For the wgmma convolution kernels the table also gives the algorithmic FLOPs of the layers they run (2 * MACs of the real
 channels, as the model defines them) and the tensor-core rate with the 3 split-fp16 terms counted: 3 * FLOPs / time against
-the H100 SXM data-sheet figure of 989 TFLOP/s dense FP16 (a share of the data-sheet peak, not a measured peak).
+the H100 SXM data-sheet figure of 989 TFLOP/s dense FP16 (a share of the data-sheet peak, not a measured peak).  Kernels bound
+by bytes rather than by the tensor pipe (the stem tail) also get their algorithmic HBM bytes against the 3.35 TB/s data sheet.
 """
 from __future__ import annotations
 
@@ -33,8 +34,7 @@ PEAK_FP16 = 989e12                       # H100 SXM data sheet, dense FP16 / BF1
 # bench's VGA input; the head chains count their 1x1 layers at 1/8 resolution.
 _B = 2 * BATCH
 _LAYERS = {
-    "conv_tc_halo_kernel<8, 8>": [(8, 8, 3, H // 2, W // 2)],                                          # block1.2
-    "conv_tc_kernel<3, 8, 32>": [(8, 24, 3, H // 4, W // 4)],                                           # block1.3
+    "stem_tail_halo_kernel": [(8, 8, 3, H // 2, W // 2), (8, 24, 3, H // 4, W // 4)],                # block1.2, block1.3
     "conv_tc_halo_kernel<32, 32>": [(24, 24, 3, H // 4, W // 4)] * 2,                                  # block2.0-1
     "conv_tc_kernel<3, 32, 64>": [(24, 64, 3, H // 8, W // 8)],                                        # block3.0
     "conv_tc_halo_kernel<64, 64>": [(64, 64, 3, H // 8, W // 8)] * 3 + [(64, 64, 3, H // 16, W // 16)] * 2,  # 3.1, fusion.0-1, 4.1-2
@@ -45,6 +45,15 @@ _LAYERS = {
     "head_chain_kernel<0>": [(64, 64, 1, H // 8, W // 8)] * 3 + [(64, 65, 1, H // 8, W // 8)],         # keypoint head
     "head_chain_kernel<1>": [(64, 64, 1, H // 8, W // 8)] * 2 + [(64, 1, 1, H // 8, W // 8)],          # reliability head
 }
+
+
+# Bandwidth-bound kernels: the HBM bytes per step their algorithm has to move, read once and written once.  The stem tail reads
+# a2 (split fp16, 32 B per half-resolution pixel) and the gray image (4 B per pixel) and writes x1s (128 B per quarter-resolution
+# pixel).
+_BYTES = {
+    "stem_tail_halo_kernel": _B * (H // 2 * W // 2 * 32 + H * W * 4 + H // 4 * W // 4 * 128),
+}
+PEAK_HBM = 3.35e12                       # H100 SXM data sheet, HBM3 bytes/s
 
 
 def algorithmic_flops(kernel: str) -> float:
@@ -143,7 +152,9 @@ def main():
         rows.append({"kernel": n, "launches_per_step": cnt / a.steps, "us_per_step": us_step, "share": us_step / total_us,
                      "algorithmic_gflop": fl / 1e9 if fl else None,
                      "split3_tflops": 3 * fl / (us_step * 1e-6) / 1e12 if fl else None,
-                     "share_of_datasheet_peak": 3 * fl / (us_step * 1e-6) / PEAK_FP16 if fl else None})
+                     "share_of_datasheet_peak": 3 * fl / (us_step * 1e-6) / PEAK_FP16 if fl else None,
+                     "algorithmic_gbytes": _BYTES[n] / 1e9 if n in _BYTES else None,
+                     "share_of_datasheet_hbm": _BYTES[n] / (us_step * 1e-6) / PEAK_HBM if n in _BYTES else None})
     wg = [r for r in rows if r["kernel"].startswith(("conv_tc", "head_chain"))]
     wg_share = sum(r["share"] for r in wg)
 
@@ -151,12 +162,14 @@ def main():
              f"step (CUDA events, profiler off, {a.steps} steps after {a.warmup} warm-up): {step_ms:.3f} ms; "
              f"summed kernel time per step under the profiler: {total_us / 1e3:.3f} ms", "",
              f"wgmma convolution + head-chain kernels: {wg_share * 100:.1f} % of the summed kernel time", "",
-             "| kernel | launches/step | us/step | share | GFLOP (alg.) | 3-term TFLOP/s | of 989 TFLOP/s data sheet |",
-             "|---|---|---|---|---|---|---|"]
+             "| kernel | launches/step | us/step | share | GFLOP (alg.) | 3-term TFLOP/s | of 989 TFLOP/s data sheet "
+             "| GB (alg.) | of 3.35 TB/s data sheet |",
+             "|---|---|---|---|---|---|---|---|---|"]
     for r in rows:
         fl = (f"{r['algorithmic_gflop']:.1f} | {r['split3_tflops']:.0f} | {r['share_of_datasheet_peak'] * 100:.0f} %"
               if r["algorithmic_gflop"] else " | | ")
-        lines.append(f"| `{r['kernel'][:110]}` | {r['launches_per_step']:g} | {r['us_per_step']:.1f} | {r['share'] * 100:.2f} % | {fl} |")
+        by = (f"{r['algorithmic_gbytes']:.2f} | {r['share_of_datasheet_hbm'] * 100:.0f} %" if r["algorithmic_gbytes"] else " | ")
+        lines.append(f"| `{r['kernel'][:110]}` | {r['launches_per_step']:g} | {r['us_per_step']:.1f} | {r['share'] * 100:.2f} % | {fl} | {by} |")
     text = "\n".join(lines) + "\n"
     with open(os.path.join(a.out, "kernels.md"), "w") as f:
         f.write(text)
