@@ -220,13 +220,14 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
     XF_RUN(launch_fuse_pyramid_split(s8a, (const __half*)ws.t16a, (const __half*)ws.t32b, sfin, B, H8, W8, st));  // model.py:146-148
     XF_RUN(launch_conv_tc(ctx, L_FU_0, sfin, B, H8, W8, sf1, nullptr, st));
     XF_RUN(launch_conv_tc(ctx, L_FU_1, sf1, B, H8, W8, sf2, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_FU_2, sf2, B, H8, W8, s8a, d_feats, st));      // fp32 feats for the samplers + split for the head
     if (g_conv_impl == 2) {
-      // fused head chains: activations stay in shared memory / registers between the 1x1 layers (head_chain_tc.cu)
-      XF_RUN(launch_head_chain(ctx, 1, s8a, B, H8, W8, d_reliability, nullptr, st));                 // model.py:151
+      // fused head chains, activations in registers between the 1x1 layers (head_chain_tc.cu): block_fusion.2 + reliability
+      // head in one kernel (fp32 feats for the samplers; the split copy stays on chip), then the keypoint head
+      XF_RUN(launch_fusion_reliability(ctx, sf2, B, H8, W8, d_feats, d_reliability, st));            // model.py:148,151
       XF_RUN(launch_head_chain(ctx, 0, d_xn, B, H8, W8, d_heat, d_kpt_logits, st));   // unfold8 (model.py:152) inside; + xfeat.py:242-247
       return XF_OK;
     }
+    XF_RUN(launch_conv_tc(ctx, L_FU_2, sf2, B, H8, W8, s8a, d_feats, st));      // fp32 feats for the samplers + split for the head
     XF_RUN(launch_conv_tc(ctx, L_HH_0, s8a, B, H8, W8, s8b, nullptr, st));                          // model.py:151
     XF_RUN(launch_conv_tc(ctx, L_HH_1, s8b, B, H8, W8, nullptr, ws.t8a, st));
     XF_RUN(launch_reliability(ctx, ws.t8a, d_reliability, (int64_t)B * H8 * W8, st));

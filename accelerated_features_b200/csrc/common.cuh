@@ -179,7 +179,9 @@ int launch_fine_mlp_tc(const xfeat_ctx* ctx, const __half* X_split, int rows_cap
 int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int B, int H, int W, __half* out_split,
                    float* out_f32, cudaStream_t st, const float* skip_xn = nullptr);
 int launch_head_chain(const xfeat_ctx* ctx, int mode, const void* in, int B, int Hc, int Wc, float* out, float* logits,
-                      cudaStream_t st);
+                      cudaStream_t st, bool reference = false);
+int launch_fusion_reliability(const xfeat_ctx* ctx, const __half* f1_split, int B, int Hc, int Wc, float* feats, float* rel,
+                              cudaStream_t st);
 int launch_split_nhwc(const float* in, __half* out, int64_t npix, int C, int CP, cudaStream_t st);
 int launch_unfold8_split(const float* xn, __half* out, int B, int Hc, int Wc, cudaStream_t st);
 int launch_stem_chain(const float* h_weights, const LayerTable& t, const float* xn, float* a1, float* a2, float* a3,

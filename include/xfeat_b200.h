@@ -389,6 +389,16 @@ XF_API int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* 
 XF_API int xfeat_debug_stem_tail(xfeat_ctx* ctx, const float* d_in, const float* d_xn, int B, int H2, int W2, void* d_out_split,
                                  void* d_scratch, size_t scratch_bytes, void* stream);
 
+/* Test hook: block_fusion.2 and the two heads as xfeat_net runs them (conv impl 2).  d_f1 (B,Hc,Wc,64) fp32 NHWC is
+ * block_fusion.1's output, split into d_scratch (>= B*Hc*Wc*512 bytes) as xfeat_debug_conv_layer_tc_ex splits it; d_xn the
+ * normalised gray image (B,8*Hc,8*Wc) fp32.  Outputs: d_feats (B,Hc,Wc,64), d_heat (B,8*Hc,8*Wc), d_rel (B*Hc*Wc) fp32 and,
+ * unless NULL, d_logits (B*Hc*Wc,65) fp32.  variant 0 (the reference): block_fusion.2 as a separate convolution, then the
+ * head chains that keep each layer's activations in shared memory; 1: what xfeat_net runs, block_fusion.2 fused into the
+ * reliability chain and both chains handing their activations over in registers. */
+XF_API int xfeat_debug_heads(xfeat_ctx* ctx, int variant, const float* d_f1, const float* d_xn, int B, int Hc, int Wc,
+                             float* d_feats, float* d_heat, float* d_rel, float* d_logits, void* d_scratch, size_t scratch_bytes,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,7 +12,7 @@ OUT/kernels.json, and prints the card's name, power limit and maximum SM clock.
 For the wgmma convolution kernels the table also gives the algorithmic FLOPs of the layers they run (2 * MACs of the real
 channels, as the model defines them) and the tensor-core rate with the 3 split-fp16 terms counted: 3 * FLOPs / time against
 the H100 SXM data-sheet figure of 989 TFLOP/s dense FP16 (a share of the data-sheet peak, not a measured peak).  Kernels bound
-by bytes rather than by the tensor pipe (the stem tail) also get their algorithmic HBM bytes against the 3.35 TB/s data sheet.
+by bytes rather than by the tensor pipe (the stem tail, the head chains) also get their algorithmic HBM bytes against the 3.35 TB/s data sheet.
 """
 from __future__ import annotations
 
@@ -38,20 +38,24 @@ _LAYERS = {
     "conv_tc_halo_kernel<32, 32>": [(24, 24, 3, H // 4, W // 4)] * 2,                                  # block2.0-1
     "conv_tc_kernel<3, 32, 64>": [(24, 64, 3, H // 8, W // 8)],                                        # block3.0
     "conv_tc_halo_kernel<64, 64>": [(64, 64, 3, H // 8, W // 8)] * 3 + [(64, 64, 3, H // 16, W // 16)] * 2,  # 3.1, fusion.0-1, 4.1-2
-    "conv_tc_kernel<1, 64, 64>": [(64, 64, 1, H // 8, W // 8)] * 2,                                    # block3.2, fusion.2
+    "conv_tc_kernel<1, 64, 64>": [(64, 64, 1, H // 8, W // 8)],                                        # block3.2
     "conv_tc_kernel<3, 64, 64>": [(64, 64, 3, H // 16, W // 16), (64, 128, 3, H // 32, W // 32)],      # block4.0, block5.0
     "conv_tc128_kernel<3>": [(128, 128, 3, H // 32, W // 32)] * 2,                                      # block5.1-2
     "conv_tc128_kernel<1>": [(128, 64, 1, H // 32, W // 32)],                                           # block5.3
-    "head_chain_kernel<0>": [(64, 64, 1, H // 8, W // 8)] * 3 + [(64, 65, 1, H // 8, W // 8)],         # keypoint head
-    "head_chain_kernel<1>": [(64, 64, 1, H // 8, W // 8)] * 2 + [(64, 1, 1, H // 8, W // 8)],          # reliability head
+    "head_chain_rf_kernel<0>": [(64, 64, 1, H // 8, W // 8)] * 3 + [(64, 65, 1, H // 8, W // 8)],      # keypoint head
+    "head_chain_rf_kernel<1>": [(64, 64, 1, H // 8, W // 8)] * 3 + [(64, 1, 1, H // 8, W // 8)],       # fusion.2 + reliability head
 }
 
 
 # Bandwidth-bound kernels: the HBM bytes per step their algorithm has to move, read once and written once.  The stem tail reads
 # a2 (split fp16, 32 B per half-resolution pixel) and the gray image (4 B per pixel) and writes x1s (128 B per quarter-resolution
-# pixel).
+# pixel).  The keypoint head reads the gray image and writes the heat-map (4 B per full-resolution pixel each); the reliability
+# head, with block_fusion.2 in front, reads fusion.1's split output (256 B per cell) and writes the fp32 features (256 B) and
+# the reliability (4 B).
 _BYTES = {
     "stem_tail_halo_kernel": _B * (H // 2 * W // 2 * 32 + H * W * 4 + H // 4 * W // 4 * 128),
+    "head_chain_rf_kernel<0>": _B * H * W * 8,
+    "head_chain_rf_kernel<1>": _B * (H // 8 * W // 8) * (256 + 256 + 4),
 }
 PEAK_HBM = 3.35e12                       # H100 SXM data sheet, HBM3 bytes/s
 
