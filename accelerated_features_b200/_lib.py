@@ -73,6 +73,7 @@ SIGNATURES = {
     "xfeat_debug_conv_layer": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p]),
     "xfeat_debug_conv_layer_tc": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
     "xfeat_debug_conv_layer_tc_ex": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz, c_p]),
+    "xfeat_debug_stem01": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
     "xfeat_debug_stem_tail": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
     "xfeat_debug_heads": (c_i, [c_p, c_i, c_p, c_p, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
 }

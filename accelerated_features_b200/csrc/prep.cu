@@ -263,6 +263,18 @@ __global__ void __launch_bounds__(256) gray_identity_u8hwc_kernel(const unsigned
   }
 }
 
+// InstanceNorm2d(1) parameters from the fp64 (sum, sum of squares) of n pixels: biased variance sum_sq / n - mean^2 (clamped at
+// 0), then mean and 1 / sqrt(var + 1e-5) rounded to float.  Both forms below call this, and every double operation is rounded on
+// its own: left to the compiler, sum_sq / n - mean * mean was contracted into an FMA in one kernel and not in the other, and for
+// a low-contrast image (mean^2 close to sum_sq / n) the two forms disagreed in the last bit of invstd.
+__device__ __forceinline__ void instnorm_params(double sum, double sum_sq, double n, float& meanf, float& invstd) {
+  const double mean = sum / n;
+  double var = __dsub_rn(sum_sq / n, __dmul_rn(mean, mean));
+  if (var < 0) var = 0;
+  meanf = (float)mean;
+  invstd = (float)(1.0 / sqrt(var + 1e-5));
+}
+
 // Gray conversion + InstanceNorm in ONE pass for images at network resolution that fit the shared memory of a thread-block
 // cluster (VGA: 1.2 MB of gray = 16 CTAs x 75 KB, two CTAs per SM so that clusters in different phases overlap).  A cluster owns an image: every CTA converts its share into shared memory
 // and sums it (fp64), the partial sums are exchanged through distributed shared memory (read in rank order by every CTA:
@@ -374,12 +386,7 @@ __global__ void __launch_bounds__(GN_THREADS, 2)
       sum += ld_dsmem_f64(ra);
       sq += ld_dsmem_f64(rb);
     }
-    const double n = (double)H * (double)W4 * 4.0;       // as instnorm_kernel
-    const double mean = sum / n;
-    double var = sq / n - mean * mean;
-    if (var < 0) var = 0;
-    sNorm[0] = (float)mean;
-    sNorm[1] = (float)(1.0 / sqrt(var + 1e-5));
+    instnorm_params(sum, sq, (double)H * (double)W4 * 4.0, sNorm[0], sNorm[1]);
     if (rank == 0) { stats[2 * b] = sum; stats[2 * b + 1] = sq; }
   }
   __syncthreads();
@@ -400,12 +407,8 @@ __global__ void __launch_bounds__(GN_THREADS, 2)
 __global__ void __launch_bounds__(256) instnorm_kernel(float* __restrict__ gray, const double* __restrict__ stats,
                                                        int HW4) {
   const int b = blockIdx.y;
-  const double n = (double)HW4 * 4.0;
-  const double mean = stats[2 * b] / n;
-  double var = stats[2 * b + 1] / n - mean * mean;
-  if (var < 0) var = 0;
-  const float meanf = (float)mean;
-  const float invstd = (float)(1.0 / sqrt(var + 1e-5));
+  float meanf, invstd;
+  instnorm_params(stats[2 * b], stats[2 * b + 1], (double)HW4 * 4.0, meanf, invstd);
   float4* p = reinterpret_cast<float4*>(gray) + (int64_t)b * HW4;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW4; i += gridDim.x * blockDim.x) {
     float4 v = p[i];
@@ -446,6 +449,9 @@ extern "C" int xfeat_resize_bilinear(const void* d_in, int dtype, int B, int C, 
   XF_REQUIRE(d_in && d_out && B > 0 && C > 0 && Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0, "resize: bad arguments");
   XF_REQUIRE((int64_t)B * C <= 65535, "resize: B*C too large for grid.z");
   XF_REQUIRE(dtype == XF_DTYPE_F32 || dtype == XF_DTYPE_U8, "resize: unsupported dtype %d", dtype);
+  // ATen copies along an axis whose size does not change, whatever the scale: scale 1 samples src == dst with weight 0 on i1
+  if (Ho == Hi) scale_h = 1.0f;
+  if (Wo == Wi) scale_w = 1.0f;
   dim3 grid(xf::cdiv(Wo, 64), xf::cdiv(Ho, 4), B * C);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == XF_DTYPE_F32)
@@ -473,6 +479,10 @@ extern "C" int xfeat_preprocess_scaled(const void* d_img, int dtype, int B, int 
   XF_REQUIRE(B > 0 && B <= 65535 && C > 0 && Hi > 0 && Wi > 0, "preprocess: bad shape");
   XF_REQUIRE(H > 0 && W > 0 && (H % 32) == 0 && (W % 32) == 0, "preprocess: H, W must be positive multiples of 32");
   XF_REQUIRE(dtype == XF_DTYPE_F32 || dtype == XF_DTYPE_U8, "preprocess: unsupported dtype %d", dtype);
+  // ATen copies along an axis whose size does not change, whatever the scale (compute_source_index_and_lambda): every form
+  // below then samples src == dst there, as the same-size fast forms do
+  if (Hi == H) sh = 1.0f;
+  if (Wi == W) sw = 1.0f;
   cudaStream_t st = (cudaStream_t)stream;
   XF_CUDA(cudaMemsetAsync(d_stats, 0, sizeof(double) * 2 * B, st));
   dim3 grid(xf::cdiv(W, 64), xf::cdiv(H, 4), B);

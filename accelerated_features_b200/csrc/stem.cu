@@ -247,6 +247,21 @@ __global__ void __launch_bounds__(128) stem01_kernel(const __grid_constant__ Ste
   }
 }
 
+// xn (B,H,W) -> block1.1's split output (B,H/2,W/2,16) fp16 [hi8|lo8] through stem01_kernel.  H, W multiples of 4.
+static int launch_stem01(const float* hw, const LayerTable& t, const float* xn, __half* out_split8, int B, int H, int W,
+                         cudaStream_t st) {
+  Stem01W P;
+  memcpy(P.w0, hw + t.w_off[L_B1_0], sizeof(P.w0));
+  memcpy(P.b0, hw + t.b_off[L_B1_0], sizeof(P.b0));
+  memcpy(P.w1, hw + t.w_off[L_B1_1], sizeof(P.w1));
+  memcpy(P.b1, hw + t.b_off[L_B1_1], sizeof(P.b1));
+  dim3 grid(cdiv(W / 4, 32), cdiv(H / 4, 4), B);
+  // (capping registers at 128 for 4 CTAs/SM measured the same 333 us as 158 registers / 3 CTAs: issue-bound, not latency-bound)
+  stem01_kernel<<<grid, 128, 0, st>>>(P, xn, out_split8, H, W);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
 static int g_stem_fused = 1;   // XFEAT_STEM_UNFUSED=1 in the environment selects the two-kernel path (A/B measurements)
 
 // xn (B,H,W) -> a1 (B,H,W,4) -> a2 (B,H/2,W/2,8) -> a3 (same,8) -> x1s (B,H/4,W/4,24) = block1(x) + skip1(x)
@@ -257,18 +272,7 @@ int launch_stem_chain(const float* h_weights, const LayerTable& t, const float* 
   const float* hw = h_weights;
   int rc;
   static const bool unfused = getenv("XFEAT_STEM_UNFUSED") != nullptr;
-  if (tc_tail && g_stem_fused && !unfused) {
-    Stem01W P;
-    memcpy(P.w0, hw + t.w_off[L_B1_0], sizeof(P.w0));
-    memcpy(P.b0, hw + t.b_off[L_B1_0], sizeof(P.b0));
-    memcpy(P.w1, hw + t.w_off[L_B1_1], sizeof(P.w1));
-    memcpy(P.b1, hw + t.b_off[L_B1_1], sizeof(P.b1));
-    dim3 grid(cdiv(W / 4, 32), cdiv(H / 4, 4), B);
-    // (capping registers at 128 for 4 CTAs/SM measured the same 333 us as 158 registers / 3 CTAs: issue-bound, not latency-bound)
-    stem01_kernel<<<grid, 128, 0, st>>>(P, xn, (__half*)a2, H, W);
-    XF_LAUNCH_CHECK();
-    return XF_OK;
-  }
+  if (tc_tail && g_stem_fused && !unfused) return launch_stem01(hw, t, xn, (__half*)a2, B, H, W, st);
   rc = launch_stem<1, 4, 1, false>(hw + t.w_off[L_B1_0], hw + t.b_off[L_B1_0], nullptr, nullptr, xn, nullptr, a1, nullptr, B, H, W, st);
   if (rc) return rc;
   rc = launch_stem<4, 8, 2, false>(hw + t.w_off[L_B1_1], hw + t.b_off[L_B1_1], nullptr, nullptr, a1, nullptr, a2,
@@ -282,3 +286,24 @@ int launch_stem_chain(const float* h_weights, const LayerTable& t, const float* 
 }
 
 }  // namespace xf
+
+// Test hook: block1.0 + block1.1 with block1.1's output split as xfeat_net hands it to block1.2 (conv impl 1 and 2).
+extern "C" int xfeat_debug_stem01(xfeat_ctx* ctx, int variant, const float* d_xn, int B, int H, int W, void* d_out_split,
+                                  void* d_scratch, size_t scratch_bytes, void* stream) {
+  XF_REQUIRE(ctx && d_xn && d_out_split && (variant == 0 || variant == 1) && B > 0 && B <= 65535 && H > 0 && W > 0 &&
+                 H % 4 == 0 && W % 4 == 0,
+             "debug_stem01: bad arguments");
+  XF_REQUIRE(variant == 1 || (d_scratch && scratch_bytes >= (size_t)B * H * W * 16),
+             "debug_stem01: variant 0 needs scratch for B*H*W*16 bytes");
+  XF_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const float* hw = ctx->h_weights;
+  const xf::LayerTable& t = ctx->table;
+  if (variant == 1) return xf::launch_stem01(hw, t, d_xn, (__half*)d_out_split, B, H, W, st);
+  float* a1 = (float*)d_scratch;
+  int rc = xf::launch_stem<1, 4, 1, false>(hw + t.w_off[xf::L_B1_0], hw + t.b_off[xf::L_B1_0], nullptr, nullptr, d_xn, nullptr,
+                                           a1, nullptr, B, H, W, st);
+  if (rc) return rc;
+  return xf::launch_stem<4, 8, 2, false>(hw + t.w_off[xf::L_B1_1], hw + t.b_off[xf::L_B1_1], nullptr, nullptr, a1, nullptr,
+                                         nullptr, (__half*)d_out_split, B, H, W, st);
+}

@@ -83,7 +83,8 @@ XF_API void xfeat_destroy(xfeat_ctx* ctx);
 /* replaces: F.interpolate(scale_factor=s, bilinear, align_corners=False) in extract_dualscale (xfeat.py:380-381)
  * (and parse_input's "/255" when div255 != 0).  Input addressed with element strides like xfeat_preprocess;
  * output NCHW fp32 (B,C,Ho,Wo) contiguous; source coordinate = (dst+0.5)*scale - 0.5 (clamped at 0), the caller
- * passes scale = float(1/scale_factor) (ATen area_pixel_compute_scale with a given scale factor). */
+ * passes scale = float(1/scale_factor) (ATen area_pixel_compute_scale with a given scale factor).  An axis whose size does not
+ * change (Ho == Hi or Wo == Wi) is copied whatever its scale, as in ATen. */
 XF_API int xfeat_resize_bilinear(const void* d_in, int dtype, int B, int C, int Hi, int Wi, int64_t stride_b,
                                  int64_t stride_c, int64_t stride_h, int64_t stride_w, int div255, float* d_out, int Ho,
                                  int Wo, float scale_h, float scale_w, void* stream);
@@ -101,7 +102,8 @@ XF_API int xfeat_preprocess(const void* d_img, int dtype, int B, int C, int Hi, 
  * scale = float(1 / s) whatever floor(Hi * s) is (xfeat.py:380-381), F.interpolate(size = ...) uses in / out (xfeat.py:239).  With
  * it extract_dualscale's resize (3 channels written and read back) folds into the gray conversion whenever the scaled size is
  * already a multiple of 32 (then preprocess_tensor's own resize is the identity): per-channel interpolation in ATen's operation
- * order, channel sum, division -- bit-identical to the two-step form. */
+ * order, channel sum, division -- bit-identical to the two-step form.  An axis with H == Hi or W == Wi is copied
+ * whatever its scale, as in ATen. */
 XF_API int xfeat_preprocess_scaled(const void* d_img, int dtype, int B, int C, int Hi, int Wi,
                             int64_t stride_b, int64_t stride_c, int64_t stride_h, int64_t stride_w, int div255,
                             int H, int W, float scale_h, float scale_w, float* d_xn, double* d_stats, void* stream);
@@ -382,6 +384,13 @@ XF_API int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float* d_i
 XF_API int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out_f32,
                                         void* d_out_split, const float* d_skip_xn, void* d_scratch, size_t scratch_bytes,
                                         void* stream);
+
+/* Test hook: block1.0 + block1.1 on the normalised gray image d_xn (B,H,W) fp32, H and W multiples of 4.  d_out_split
+ * (B,H/2,W/2,16) fp16 [hi(8) | lo(8)] is block1.1's output split as block1.2 reads it.  variant 0 (the reference): block1.0
+ * into d_scratch (>= B*H*W*16 bytes, its (B,H,W,4) fp32 output), then block1.1, one direct convolution each; 1: what xfeat_net
+ * runs under conv impl 1 and 2, both layers in one kernel that recomputes block1.0 in registers (d_scratch unused). */
+XF_API int xfeat_debug_stem01(xfeat_ctx* ctx, int variant, const float* d_xn, int B, int H, int W, void* d_out_split,
+                              void* d_scratch, size_t scratch_bytes, void* stream);
 
 /* Test hook: the stem tail xfeat_net runs (block1.2, then block1.3 + skip1, in one kernel).  d_in (B,H2,W2,8) fp32 NHWC is
  * block1.1's output, split into d_scratch (>= B*H2*W2*32 bytes) as xfeat_debug_conv_layer_tc_ex splits it; d_xn the normalised
