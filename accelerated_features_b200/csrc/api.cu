@@ -12,7 +12,7 @@ namespace xf {
 
 static thread_local char g_err[1024] = "";
 unsigned long long g_launches = 0;
-int g_conv_impl = 2;  // 0 = fp32 CUDA-core convs everywhere, 1 = wgmma for the tensor-core layers, 2 = 1 + halo-patch 3x3 (default)
+int g_conv_impl = 2;  // 0 = fp32 CUDA-core convs everywhere, 2 = the tensor-core schedule (default)
 
 // (device, kernel) -> largest dynamic shared-memory size opted into so far
 int ensure_dyn_smem(const void* func, size_t bytes) {
@@ -117,7 +117,7 @@ extern "C" int xfeat_create(xfeat_ctx** out, int device, const float* packed_hos
   return XF_OK;
 }
 
-extern "C" void xfeat_set_conv_impl(int impl) { xf::g_conv_impl = (impl < 0 || impl > 2) ? 1 : impl; }
+extern "C" void xfeat_set_conv_impl(int impl) { xf::g_conv_impl = impl == 0 ? 0 : 2; }
 extern "C" int xfeat_get_conv_impl(void) { return xf::g_conv_impl; }
 
 extern "C" void xfeat_destroy(xfeat_ctx* ctx) {
@@ -158,7 +158,7 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
   if (g_conv_impl == 0) {
     // ------------------------------ all layers on the fp32 CUDA-core kernels ------------------------------
     // block1 + skip1 -> x1 + skip1(x)                                            model.py:139-140
-    XF_RUN(launch_stem_chain(ctx->h_weights, ctx->table, d_xn, ws.a1, ws.a2, ws.a3, ws.x1s, nullptr, B, H, W, st));
+    XF_RUN(launch_stem_chain(ctx->h_weights, ctx->table, d_xn, ws.a1, ws.a2, ws.a3, ws.x1s, B, H, W, st));
     XF_RUN(launch_conv_layer(ctx, L_B2_0, ws.x1s, IN_NHWC, B, H4, W4, ws.t4a, st));                  // block2, model.py:140
     XF_RUN(launch_conv_layer(ctx, L_B2_1, ws.t4a, IN_NHWC, B, H4, W4, ws.x2, st));
     XF_RUN(launch_conv_layer(ctx, L_B3_0, ws.x2, IN_NHWC, B, H4, W4, ws.t8a, st));                   // block3, model.py:141
@@ -168,41 +168,11 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
     XF_RUN(launch_conv_layer(ctx, L_B4_1, ws.t16a, IN_NHWC, B, H16, W16, ws.t16b, st));
     XF_RUN(launch_conv_layer(ctx, L_B4_2, ws.t16b, IN_NHWC, B, H16, W16, ws.x4, st));
     XF_RUN(launch_conv_layer(ctx, L_B5_0, ws.x4, IN_NHWC, B, H16, W16, ws.t32a, st));                // block5, model.py:143
-  } else {
-    // ---- block2 .. block5.0 on the tensor cores (wgmma); activations between tensor-core layers travel as split fp16 [hi | lo] ----
-    __half *s4a = (__half*)ws.x1s, *s4b = (__half*)ws.t4a, *s4c = (__half*)ws.x2;
-    __half *s8a = (__half*)ws.t8a, *s8b = (__half*)ws.t8b, *s16a = (__half*)ws.t16a, *s16b = (__half*)ws.t16b;
-    if (g_conv_impl == 2) {
-      // block1.0/1.1 on CUDA cores (K = 9 / 36), then block1.2 and block1.3 + skip1 in one tensor-core kernel with 32-byte
-      // operand rows [hi(8)|lo(8)], block1.2's output kept in shared memory        model.py:43-48,139-140
-      XF_RUN(launch_stem_chain(ctx->h_weights, ctx->table, d_xn, ws.a1, ws.a2, ws.a3, nullptr, nullptr, B, H, W, st, 1));
-      XF_RUN(launch_stem_tail_halo(ctx, (const __half*)ws.a2, d_xn, B, H / 2, W / 2, s4a, st));
-    } else {
-      XF_RUN(launch_stem_chain(ctx->h_weights, ctx->table, d_xn, ws.a1, ws.a2, ws.a3, nullptr, s4a, B, H, W, st));
-    }
-    XF_RUN(launch_conv_tc(ctx, L_B2_0, s4a, B, H4, W4, s4b, nullptr, st));                           // block2, model.py:140
-    XF_RUN(launch_conv_tc(ctx, L_B2_1, s4b, B, H4, W4, s4c, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B3_0, s4c, B, H4, W4, s8a, nullptr, st));                           // block3 (stride 2), model.py:141
-    XF_RUN(launch_conv_tc(ctx, L_B3_1, s8a, B, H8, W8, s8b, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B3_2, s8b, B, H8, W8, s8a, nullptr, st));     // x3 stays split: block4.0 and the fusion read it
-    XF_RUN(launch_conv_tc(ctx, L_B4_0, s8a, B, H8, W8, s16a, nullptr, st));                          // block4 (stride 2), model.py:142
-    XF_RUN(launch_conv_tc(ctx, L_B4_1, s16a, B, H16, W16, s16b, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B4_2, s16b, B, H16, W16, s16a, nullptr, st)); // x4 stays split: block5.0 and the fusion read it
-    // block5: 128 channels, split tensors are [hi(128) | lo(128)] = 512 B per pixel            model.py:143
-    __half *s32a = (__half*)ws.t32a, *s32b = (__half*)ws.t32b;
-    XF_RUN(launch_conv_tc(ctx, L_B5_0, s16a, B, H16, W16, s32a, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B5_1, s32a, B, H32, W32, s32b, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B5_2, s32b, B, H32, W32, s32a, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_B5_3, s32a, B, H32, W32, s32b, nullptr, st));  // x5 (64 ch) split, for the fusion
-  }
-  if (g_conv_impl == 0) {   // rest of block5 on the fp32 CUDA-core kernel                  model.py:143
     XF_RUN(launch_conv_layer(ctx, L_B5_1, ws.t32a, IN_NHWC, B, H32, W32, ws.t32b, st));
     XF_RUN(launch_conv_layer(ctx, L_B5_2, ws.t32b, IN_NHWC, B, H32, W32, ws.t32a, st));
     XF_RUN(launch_conv_layer(ctx, L_B5_3, ws.t32a, IN_NHWC, B, H32, W32, ws.x5, st));
-  }
-  if (g_conv_impl == 0) {
     // pyramid fusion                                                             model.py:146-148
-    XF_RUN(launch_fuse_pyramid(ws.x3, ws.x4, ws.x5, ws.fin, nullptr, B, H8, W8, st));
+    XF_RUN(launch_fuse_pyramid(ws.x3, ws.x4, ws.x5, ws.fin, B, H8, W8, st));
     XF_RUN(launch_conv_layer(ctx, L_FU_0, ws.fin, IN_NHWC, B, H8, W8, ws.f1, st));
     XF_RUN(launch_conv_layer(ctx, L_FU_1, ws.f1, IN_NHWC, B, H8, W8, ws.f2, st));
     XF_RUN(launch_conv_layer(ctx, L_FU_2, ws.f2, IN_NHWC, B, H8, W8, d_feats, st));
@@ -215,28 +185,37 @@ extern "C" int xfeat_net(xfeat_ctx* ctx, const float* d_xn, int B, int H, int W,
     XF_RUN(launch_conv_layer(ctx, L_KH_1, ws.t8a, IN_NHWC, B, H8, W8, ws.t8b, st));
     XF_RUN(launch_conv_layer(ctx, L_KH_2, ws.t8b, IN_NHWC, B, H8, W8, ws.t8a, st));
     XF_RUN(launch_kpt_softmax(ctx, ws.t8a, d_heat, d_kpt_logits, B, H8, W8, st));
-  } else {
-    __half *s8a = (__half*)ws.t8a, *s8b = (__half*)ws.t8b, *sfin = (__half*)ws.fin, *sf1 = (__half*)ws.f1, *sf2 = (__half*)ws.f2;
-    XF_RUN(launch_fuse_pyramid_split(s8a, (const __half*)ws.t16a, (const __half*)ws.t32b, sfin, B, H8, W8, st));  // model.py:146-148
-    XF_RUN(launch_conv_tc(ctx, L_FU_0, sfin, B, H8, W8, sf1, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_FU_1, sf1, B, H8, W8, sf2, nullptr, st));
-    if (g_conv_impl == 2) {
-      // fused head chains, activations in registers between the 1x1 layers (head_chain_tc.cu): block_fusion.2 + reliability
-      // head in one kernel (fp32 feats for the samplers; the split copy stays on chip), then the keypoint head
-      XF_RUN(launch_fusion_reliability(ctx, sf2, B, H8, W8, d_feats, d_reliability, st));            // model.py:148,151
-      XF_RUN(launch_head_chain(ctx, 0, d_xn, B, H8, W8, d_heat, d_kpt_logits, st));   // unfold8 (model.py:152) inside; + xfeat.py:242-247
-      return XF_OK;
-    }
-    XF_RUN(launch_conv_tc(ctx, L_FU_2, sf2, B, H8, W8, s8a, d_feats, st));      // fp32 feats for the samplers + split for the head
-    XF_RUN(launch_conv_tc(ctx, L_HH_0, s8a, B, H8, W8, s8b, nullptr, st));                          // model.py:151
-    XF_RUN(launch_conv_tc(ctx, L_HH_1, s8b, B, H8, W8, nullptr, ws.t8a, st));
-    XF_RUN(launch_reliability(ctx, ws.t8a, d_reliability, (int64_t)B * H8 * W8, st));
-    XF_RUN(launch_unfold8_split(d_xn, s8b, B, H8, W8, st));                                          // model.py:152
-    XF_RUN(launch_conv_tc(ctx, L_KH_0, s8b, B, H8, W8, s8a, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_KH_1, s8a, B, H8, W8, s8b, nullptr, st));
-    XF_RUN(launch_conv_tc(ctx, L_KH_2, s8b, B, H8, W8, nullptr, ws.t8a, st));
-    XF_RUN(launch_kpt_softmax(ctx, ws.t8a, d_heat, d_kpt_logits, B, H8, W8, st));
+    return XF_OK;
   }
+  // ---- tensor-core schedule (wgmma); activations between tensor-core layers travel as split fp16 [hi | lo] ----
+  __half *s4a = (__half*)ws.x1s, *s4b = (__half*)ws.t4a, *s4c = (__half*)ws.x2;
+  __half *s8a = (__half*)ws.t8a, *s8b = (__half*)ws.t8b, *s16a = (__half*)ws.t16a, *s16b = (__half*)ws.t16b;
+  // block1.0/1.1 on CUDA cores (K = 9 / 36) in one kernel, then block1.2 and block1.3 + skip1 in one tensor-core kernel with
+  // 32-byte operand rows [hi(8)|lo(8)], block1.2's output kept in shared memory        model.py:43-48,139-140
+  XF_RUN(launch_stem01(ctx->h_weights, ctx->table, d_xn, (__half*)ws.a2, B, H, W, st));
+  XF_RUN(launch_stem_tail_halo(ctx, (const __half*)ws.a2, d_xn, B, H / 2, W / 2, s4a, st));
+  XF_RUN(launch_conv_tc(ctx, L_B2_0, s4a, B, H4, W4, s4b, nullptr, st));                             // block2, model.py:140
+  XF_RUN(launch_conv_tc(ctx, L_B2_1, s4b, B, H4, W4, s4c, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B3_0, s4c, B, H4, W4, s8a, nullptr, st));                             // block3 (stride 2), model.py:141
+  XF_RUN(launch_conv_tc(ctx, L_B3_1, s8a, B, H8, W8, s8b, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B3_2, s8b, B, H8, W8, s8a, nullptr, st));       // x3 stays split: block4.0 and the fusion read it
+  XF_RUN(launch_conv_tc(ctx, L_B4_0, s8a, B, H8, W8, s16a, nullptr, st));                            // block4 (stride 2), model.py:142
+  XF_RUN(launch_conv_tc(ctx, L_B4_1, s16a, B, H16, W16, s16b, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B4_2, s16b, B, H16, W16, s16a, nullptr, st));   // x4 stays split: block5.0 and the fusion read it
+  // block5: 128 channels, split tensors are [hi(128) | lo(128)] = 512 B per pixel            model.py:143
+  __half *s32a = (__half*)ws.t32a, *s32b = (__half*)ws.t32b;
+  XF_RUN(launch_conv_tc(ctx, L_B5_0, s16a, B, H16, W16, s32a, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B5_1, s32a, B, H32, W32, s32b, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B5_2, s32b, B, H32, W32, s32a, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_B5_3, s32a, B, H32, W32, s32b, nullptr, st));    // x5 (64 ch) split, for the fusion
+  __half *sfin = (__half*)ws.fin, *sf1 = (__half*)ws.f1, *sf2 = (__half*)ws.f2;
+  XF_RUN(launch_fuse_pyramid_split(s8a, (const __half*)ws.t16a, (const __half*)ws.t32b, sfin, B, H8, W8, st));  // model.py:146-148
+  XF_RUN(launch_conv_tc(ctx, L_FU_0, sfin, B, H8, W8, sf1, nullptr, st));
+  XF_RUN(launch_conv_tc(ctx, L_FU_1, sf1, B, H8, W8, sf2, nullptr, st));
+  // fused head chains, activations in registers between the 1x1 layers (head_chain_tc.cu): block_fusion.2 + reliability
+  // head in one kernel (fp32 feats for the samplers; the split copy stays on chip), then the keypoint head
+  XF_RUN(launch_fusion_reliability(ctx, sf2, B, H8, W8, d_feats, d_reliability, st));                // model.py:148,151
+  XF_RUN(launch_head_chain(ctx, 0, d_xn, B, H8, W8, d_heat, d_kpt_logits, st));   // unfold8 (model.py:152) inside; + xfeat.py:242-247
 #undef XF_RUN
   return XF_OK;
 }

@@ -163,8 +163,8 @@ struct xfeat_ctx {
 namespace xf {
 enum { IN_NHWC = 0, IN_UNFOLD8 = 1 };
 int launch_conv_layer(const xfeat_ctx* ctx, int layer, const float* in, int in_mode, int B, int Hi, int Wi,
-                      float* out, cudaStream_t st, const int* n_live = nullptr, __half* out_split = nullptr);
-extern int g_conv_impl;  // 0 = fp32 CUDA cores, 1 = wgmma (per-tap operand loads), 2 = wgmma + halo-patch reuse for 3x3/s1
+                      float* out, cudaStream_t st, const int* n_live = nullptr);
+extern int g_conv_impl;  // 0 = fp32 CUDA cores, 2 = the tensor-core schedule (default)
 bool conv_tc_eligible(int layer);
 int launch_conv_tc_halo(const xfeat_ctx* ctx, int layer, const __half* in_split, int B, int H, int W, __half* out_split,
                         float* out_f32, cudaStream_t st);
@@ -183,11 +183,11 @@ int launch_head_chain(const xfeat_ctx* ctx, int mode, const void* in, int B, int
 int launch_fusion_reliability(const xfeat_ctx* ctx, const __half* f1_split, int B, int Hc, int Wc, float* feats, float* rel,
                               cudaStream_t st);
 int launch_split_nhwc(const float* in, __half* out, int64_t npix, int C, int CP, cudaStream_t st);
-int launch_unfold8_split(const float* xn, __half* out, int B, int Hc, int Wc, cudaStream_t st);
+int launch_stem01(const float* hw, const LayerTable& t, const float* xn, __half* out_split8, int B, int H, int W,
+                  cudaStream_t st);
 int launch_stem_chain(const float* h_weights, const LayerTable& t, const float* xn, float* a1, float* a2, float* a3,
-                      float* x1s, __half* x1s_split32, int B, int H, int W, cudaStream_t st, int tc_tail = 0);
-int launch_fuse_pyramid(const float* x3, const float* x4, const float* x5, float* out, __half* out_split, int B, int H3,
-                        int W3, cudaStream_t st);
+                      float* x1s, int B, int H, int W, cudaStream_t st);
+int launch_fuse_pyramid(const float* x3, const float* x4, const float* x5, float* out, int B, int H3, int W3, cudaStream_t st);
 int launch_fuse_pyramid_split(const __half* x3, const __half* x4, const __half* x5, __half* out_split, int B, int H3, int W3,
                               cudaStream_t st);
 int launch_reliability(const xfeat_ctx* ctx, const float* t, float* out, int64_t npix, cudaStream_t st);

@@ -58,8 +58,7 @@ __global__ void __launch_bounds__(C::THREADS) conv_simt_kernel(const float* __re
                                                                const float* __restrict__ wgt,
                                                                const float* __restrict__ bias, float* __restrict__ out,
                                                                int Hi, int Wi, int Ho, int Wo,
-                                                               const int* __restrict__ n_live_cols,
-                                                               __half* __restrict__ out_split) {
+                                                               const int* __restrict__ n_live_cols) {
   constexpr int CIN = C::CIN, COUT = C::COUT, CT = C::CT, KS = C::KS, S = C::S, TH = C::TH, TW = C::TW, PM = C::PM;
   constexpr int KC = C::KC, NCG = C::NCG, NPGX = C::NPGX, PH = C::PH, PW = C::PW, PWP = C::PWP, NA4 = C::NA4;
   extern __shared__ __align__(16) float smem[];
@@ -154,25 +153,9 @@ __global__ void __launch_bounds__(C::THREADS) conv_simt_kernel(const float* __re
           if (C::RELU) v = fmaxf(v, 0.f);
           r[n] = v;
         }
-        if (COUT == 64 && out_split != nullptr) {
-          // feed a tensor-core layer: x = hi + lo in fp16, NHWC with [hi(64) | lo(64)] per pixel (conv_tc.cu)
-          __half* sp = out_split + (((int64_t)b * Ho + oy) * Wo + ox) * 128;
-          __half2 h[4], l[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            h[j] = __floats2half2_rn(r[2 * j], r[2 * j + 1]);
-            const float2 hf = __half22float2(h[j]);
-            l[j] = __floats2half2_rn(r[2 * j] - hf.x, r[2 * j + 1] - hf.y);
-          }
-          *reinterpret_cast<uint2*>(sp + coA) = make_uint2(*reinterpret_cast<uint32_t*>(&h[0]), *reinterpret_cast<uint32_t*>(&h[1]));
-          *reinterpret_cast<uint2*>(sp + coB) = make_uint2(*reinterpret_cast<uint32_t*>(&h[2]), *reinterpret_cast<uint32_t*>(&h[3]));
-          *reinterpret_cast<uint2*>(sp + 64 + coA) = make_uint2(*reinterpret_cast<uint32_t*>(&l[0]), *reinterpret_cast<uint32_t*>(&l[1]));
-          *reinterpret_cast<uint2*>(sp + 64 + coB) = make_uint2(*reinterpret_cast<uint32_t*>(&l[2]), *reinterpret_cast<uint32_t*>(&l[3]));
-        } else {
-          float* op = out + (((int64_t)b * Ho + oy) * Wo + ox) * COUT + co_base;
-          *reinterpret_cast<float4*>(op + coA) = make_float4(r[0], r[1], r[2], r[3]);
-          *reinterpret_cast<float4*>(op + coB) = make_float4(r[4], r[5], r[6], r[7]);
-        }
+        float* op = out + (((int64_t)b * Ho + oy) * Wo + ox) * COUT + co_base;
+        *reinterpret_cast<float4*>(op + coA) = make_float4(r[0], r[1], r[2], r[3]);
+        *reinterpret_cast<float4*>(op + coB) = make_float4(r[4], r[5], r[6], r[7]);
       }
     }
   }
@@ -180,13 +163,13 @@ __global__ void __launch_bounds__(C::THREADS) conv_simt_kernel(const float* __re
 
 template <class C>
 static int launch_cfg(const float* in, const float* w, const float* bias, float* out, int B, int Hi, int Wi,
-                      cudaStream_t st, const int* n_live = nullptr, __half* out_split = nullptr) {
+                      cudaStream_t st, const int* n_live = nullptr) {
   const int Ho = (C::KS == 3) ? (Hi + 2 - 3) / C::S + 1 : Hi / C::S;
   const int Wo = (C::KS == 3) ? (Wi + 2 - 3) / C::S + 1 : Wi / C::S;
   XF_DYN_SMEM(conv_simt_kernel<C>, C::SMEM);
   XF_REQUIRE(B <= 65535, "conv: batch too large for grid.z");
   dim3 grid(cdiv(Ho, C::TH) * cdiv(Wo, C::TW), C::COUT / C::CT, B);
-  conv_simt_kernel<C><<<grid, C::THREADS, C::SMEM, st>>>(in, w, bias, out, Hi, Wi, Ho, Wo, n_live, out_split);
+  conv_simt_kernel<C><<<grid, C::THREADS, C::SMEM, st>>>(in, w, bias, out, Hi, Wi, Ho, Wo, n_live);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }
@@ -201,7 +184,7 @@ static int launch_pointwise(const float* in, const float* w, const float* bias, 
 }
 
 int launch_conv_layer(const xfeat_ctx* ctx, int layer, const float* in, int in_mode, int B, int Hi, int Wi, float* out,
-                      cudaStream_t st, const int* n_live, __half* out_split) {
+                      cudaStream_t st, const int* n_live) {
   const float* w = ctx->d_weights + ctx->table.w_off[layer];
   const float* bi = ctx->d_weights + ctx->table.b_off[layer];
   const int64_t npix = (int64_t)B * Hi * Wi;
@@ -210,13 +193,13 @@ int launch_conv_layer(const xfeat_ctx* ctx, int layer, const float* in, int in_m
     case L_B2_1:  // 24->24 3x3 s1 at 1/4 res
       return launch_cfg<ConvCfg<24, 24, 24, 3, 1, 16, 32, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st);
     case L_B3_0:  // 24->64 3x3 s2 -> 1/8 res
-      return launch_cfg<ConvCfg<24, 64, 64, 3, 2, 10, 16, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st, nullptr, out_split);
+      return launch_cfg<ConvCfg<24, 64, 64, 3, 2, 10, 16, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st);
     case L_B3_1:
     case L_FU_0:
     case L_FU_1:  // 64->64 3x3 s1 at 1/8 res (40% of all FLOPs)
       return launch_cfg<ConvCfg<64, 64, 64, 3, 1, 12, 16, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st);
     case L_B4_0:  // 64->64 3x3 s2 -> 1/16 res
-      return launch_cfg<ConvCfg<64, 64, 64, 3, 2, 5, 40, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st, nullptr, out_split);
+      return launch_cfg<ConvCfg<64, 64, 64, 3, 2, 5, 40, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st);
     case L_B4_1:
     case L_B4_2:  // 64->64 3x3 s1 at 1/16 res
       return launch_cfg<ConvCfg<64, 64, 64, 3, 1, 6, 40, 8, 8, IN_NHWC, 1>>(in, w, bi, out, B, Hi, Wi, st);

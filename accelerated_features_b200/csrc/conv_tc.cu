@@ -1,7 +1,7 @@
-// 64->64 convolutions (3x3 pad 1 / 1x1, stride 1) as implicit GEMM on the Hopper tensor cores:
-// TMA-fed shared-memory operands, wgmma with fp32 register accumulators, bias+ReLU epilogue.
-// Used for block3.1/3.2, block4.1/4.2, block_fusion.0-2, heatmap_head.0-1, keypoint_head.0-2 (model.py:55-92) -- 48 % of
-// the network's FLOPs.
+// Convolutions as implicit GEMM on the Hopper tensor cores: TMA-fed shared-memory operands,
+// wgmma with fp32 register accumulators, bias+ReLU epilogue.  xfeat_net runs the stride-2 layers (block3.0, block4.0,
+// block5.0), the 1x1 block3.2 and the 128-channel block5.1-5.3 here (model.py:55-71); launch_conv_tc sends the 3x3 stride-1
+// layers to the halo-patch kernel (conv_tc_halo.cu).
 //
 // fp32-equivalent precision by operand splitting (SURVEY 7.2: single-pass TF32/BF16/FP16 moves keypoints and misses the
 // 1e-3 descriptor tolerance; 3-term splits reproduce the fp32 result):  x = hi + lo in fp16, w*2^k = whi + wlo in fp16,
@@ -386,7 +386,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv_tc128_kernel(const __grid_
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// helpers: fp32 NHWC (64 ch) -> split fp16 NHWC (128 halves); unfold8 + split of the normalised gray image
+// helper: fp32 NHWC -> split fp16 NHWC [hi | lo]
 // ---------------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo) {
   __half2 h[4], l[4];
@@ -422,33 +422,8 @@ __global__ void __launch_bounds__(256) split_nhwc_kernel(const float* __restrict
   reinterpret_cast<uint4*>(out + pix * 2 * CP)[G + g] = lo;
 }
 
-// XFeatModel._unfold2d(x, 8) (model.py:113-120) fused with the split: channel 8i+j of cell (h,w) = xn[8h+i, 8w+j].
-__global__ void __launch_bounds__(256) unfold8_split_kernel(const float* __restrict__ xn, __half* __restrict__ out, int Hc,
-                                                            int Wc, int64_t ncell) {
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;  // one thread per (cell, row i)
-  if (gid >= ncell * 8) return;
-  const int64_t cell = gid >> 3;
-  const int i = (int)(gid & 7);
-  const int64_t b = cell / ((int64_t)Hc * Wc);
-  const int rem = (int)(cell - b * Hc * Wc);
-  const int h = rem / Wc, w = rem - h * Wc;
-  const float* p = xn + ((int64_t)b * Hc * 8 + h * 8 + i) * (Wc * 8) + w * 8;
-  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), c = __ldg(reinterpret_cast<const float4*>(p) + 1);
-  const float x[8] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w};
-  uint4 hi, lo;
-  split8(x, hi, lo);
-  reinterpret_cast<uint4*>(out + cell * 128)[i] = hi;
-  reinterpret_cast<uint4*>(out + cell * 128)[8 + i] = lo;
-}
-
 int launch_split_nhwc(const float* in, __half* out, int64_t npix, int C, int CP, cudaStream_t st) {
   split_nhwc_kernel<<<(unsigned)((npix * (CP / 8) + 255) / 256), 256, 0, st>>>(in, out, npix, C, CP);
-  XF_LAUNCH_CHECK();
-  return XF_OK;
-}
-int launch_unfold8_split(const float* xn, __half* out, int B, int Hc, int Wc, cudaStream_t st) {
-  const int64_t ncell = (int64_t)B * Hc * Wc;
-  unfold8_split_kernel<<<(unsigned)((ncell * 8 + 255) / 256), 256, 0, st>>>(xn, out, Hc, Wc, ncell);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }
@@ -604,8 +579,7 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
   TcLayer c;
   XF_REQUIRE(tc_layer_cfg(layer, c) && ctx->d_tcw, "conv_tc: layer %d not prepared for the tensor-core path", layer);
   XF_REQUIRE(out_split || out_f32, "conv_tc: no output");
-  XF_REQUIRE(!(c.cinp == 8 && c.nout == 8 && g_conv_impl != 2), "conv_tc: block1.2 runs on the halo kernel only (conv impl 2)");
-  if (g_conv_impl == 2 && kLayers[layer].ks == 3 && kLayers[layer].stride == 1 && c.ntiles == 1 && c.cinp == c.nout)
+  if (kLayers[layer].ks == 3 && kLayers[layer].stride == 1 && c.ntiles == 1 && c.cinp == c.nout)
     return launch_conv_tc_halo(ctx, layer, in_split, B, Hin, Win, out_split, out_f32, st);
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) {
@@ -694,7 +668,6 @@ int launch_conv_tc(const xfeat_ctx* ctx, int layer, const __half* in_split, int 
     P.n_real = sp.cout - nt * c.nout < c.nout ? sp.cout - nt * c.nout : c.nout;
     if (sp.ks == 3 && c.cinp == 64 && c.nout == 64) rc = launch_tc_cfg<3, 64, 64>(P, grid, st);
     else if (sp.ks == 1 && c.cinp == 64 && c.nout == 64) rc = launch_tc_cfg<1, 64, 64>(P, grid, st);
-    else if (sp.ks == 3 && c.cinp == 32 && c.nout == 32) rc = launch_tc_cfg<3, 32, 32>(P, grid, st);
     else if (sp.ks == 3 && c.cinp == 32 && c.nout == 64) rc = launch_tc_cfg<3, 32, 64>(P, grid, st);
     else if (sp.ks == 3 && c.cinp == 8 && c.nout == 32) rc = launch_tc_cfg<3, 8, 32>(P, grid, st);
     else {

@@ -8,9 +8,8 @@ namespace xf {
 
 // out = x3 + up2(x4) + up4(x5)   (NHWC, 64 channels; bilinear, align_corners=False; F.interpolate to x3's size)
 __global__ void __launch_bounds__(256) fuse_pyramid_kernel(const float* __restrict__ x3, const float* __restrict__ x4,
-                                                           const float* __restrict__ x5, float* __restrict__ out,
-                                                           __half* __restrict__ out_split, int H3, int W3, int H4, int W4,
-                                                           int H5, int W5, int64_t total4) {
+                                                           const float* __restrict__ x5, float* __restrict__ out, int H3,
+                                                           int W3, int H4, int W4, int H5, int W5, int64_t total4) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total4) return;
   const int c4 = (int)(i & 15);
@@ -36,16 +35,7 @@ __global__ void __launch_bounds__(256) fuse_pyramid_kernel(const float* __restri
     r.x += XF_BIL(x); r.y += XF_BIL(y); r.z += XF_BIL(z); r.w += XF_BIL(w);
 #undef XF_BIL
   }
-  if (out_split) {   // consumer is a tensor-core layer: [hi(64) | lo(64)] fp16 per pixel
-    const __half2 h0 = __floats2half2_rn(r.x, r.y), h1 = __floats2half2_rn(r.z, r.w);
-    const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-    const __half2 l0 = __floats2half2_rn(r.x - f0.x, r.y - f0.y), l1 = __floats2half2_rn(r.z - f1.x, r.w - f1.y);
-    __half* sp = out_split + (i >> 4) * 128 + c4 * 4;
-    *reinterpret_cast<uint2*>(sp) = make_uint2(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1));
-    *reinterpret_cast<uint2*>(sp + 64) = make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
-  } else {
-    reinterpret_cast<float4*>(out)[i] = r;
-  }
+  reinterpret_cast<float4*>(out)[i] = r;
 }
 
 // reliability = sigmoid(t . w + b), t: (npix,64) NHWC. 8 lanes per pixel, 8 channels per lane.
@@ -210,11 +200,10 @@ int launch_fuse_pyramid_split(const __half* x3, const __half* x4, const __half* 
   return XF_OK;
 }
 
-int launch_fuse_pyramid(const float* x3, const float* x4, const float* x5, float* out, __half* out_split, int B, int H3,
-                        int W3, cudaStream_t st) {
+int launch_fuse_pyramid(const float* x3, const float* x4, const float* x5, float* out, int B, int H3, int W3, cudaStream_t st) {
   const int64_t total4 = (int64_t)B * H3 * W3 * 16;
-  fuse_pyramid_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(x3, x4, x5, out, out_split, H3, W3, H3 / 2, W3 / 2,
-                                                                         H3 / 4, W3 / 4, total4);
+  fuse_pyramid_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(x3, x4, x5, out, H3, W3, H3 / 2, W3 / 2, H3 / 4, W3 / 4,
+                                                                         total4);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }

@@ -35,7 +35,7 @@ template <int CIN, int COUT, int S, bool SKIP>
 __global__ void __launch_bounds__(128) stem_conv_kernel(const __grid_constant__ StemW<CIN, COUT> P,
                                                         const __grid_constant__ SkipW K,
                                                         const float* __restrict__ in, const float* __restrict__ xn,
-                                                        float* __restrict__ out, __half* __restrict__ out_split32, int Hi,
+                                                        float* __restrict__ out, __half* __restrict__ out_split8, int Hi,
                                                         int Wi, int Ho, int Wo) {
   const int ox = blockIdx.x * 32 + (threadIdx.x & 31);
   const int oy = blockIdx.y * 4 + (threadIdx.x >> 5);
@@ -85,31 +85,8 @@ __global__ void __launch_bounds__(128) stem_conv_kernel(const __grid_constant__ 
     if constexpr (SKIP) v += fmaf(skipv, K.w[co], K.b[co]);
     res[co] = v;
   }
-  if constexpr (COUT == 24) {
-    if (out_split32 != nullptr) {
-      // feed the tensor-core block2: [hi(32) | lo(32)] fp16 per pixel, channels 24..31 zero (conv_tc.cu)
-      uint4* sp = reinterpret_cast<uint4*>(out_split32 + (((int64_t)b * Ho + oy) * Wo + ox) * 64);
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t hw[4], lw[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int c = 8 * g + 2 * j;
-          const float x0 = (c < 24) ? res[c < 24 ? c : 0] : 0.f, x1 = (c + 1 < 24) ? res[c + 1 < 24 ? c + 1 : 0] : 0.f;
-          const __half2 h = __floats2half2_rn(x0, x1);
-          const float2 hf = __half22float2(h);
-          const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
-          hw[j] = *reinterpret_cast<const uint32_t*>(&h);
-          lw[j] = *reinterpret_cast<const uint32_t*>(&l);
-        }
-        sp[g] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        sp[4 + g] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      }
-      return;
-    }
-  }
   if constexpr (COUT == 8) {
-    if (out_split32 != nullptr) {
+    if (out_split8 != nullptr) {
       // feed the tensor-core block1.2: [hi(8) | lo(8)] fp16 per pixel = 32 bytes (conv_tc_halo.cu, 32-byte operand rows)
       uint32_t hw[4], lw[4];
 #pragma unroll
@@ -120,7 +97,7 @@ __global__ void __launch_bounds__(128) stem_conv_kernel(const __grid_constant__ 
         hw[j] = *reinterpret_cast<const uint32_t*>(&h);
         lw[j] = *reinterpret_cast<const uint32_t*>(&l);
       }
-      uint4* sp = reinterpret_cast<uint4*>(out_split32 + (((int64_t)b * Ho + oy) * Wo + ox) * 16);
+      uint4* sp = reinterpret_cast<uint4*>(out_split8 + (((int64_t)b * Ho + oy) * Wo + ox) * 16);
       sp[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
       sp[1] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
       return;
@@ -134,7 +111,7 @@ __global__ void __launch_bounds__(128) stem_conv_kernel(const __grid_constant__ 
 
 template <int CIN, int COUT, int S, bool SKIP>
 static int launch_stem(const float* hw, const float* hb, const float* sw, const float* sb, const float* in,
-                       const float* xn, float* out, __half* out_split32, int B, int Hi, int Wi, cudaStream_t st) {
+                       const float* xn, float* out, __half* out_split8, int B, int Hi, int Wi, cudaStream_t st) {
   StemW<CIN, COUT> P;
   memcpy(P.w, hw, sizeof(P.w));
   memcpy(P.b, hb, sizeof(P.b));
@@ -143,7 +120,7 @@ static int launch_stem(const float* hw, const float* hb, const float* sw, const 
   if (SKIP) { memcpy(K.w, sw, sizeof(K.w)); memcpy(K.b, sb, sizeof(K.b)); }
   const int Ho = Hi / S, Wo = Wi / S;
   dim3 grid(cdiv(Wo, 32), cdiv(Ho, 4), B);
-  stem_conv_kernel<CIN, COUT, S, SKIP><<<grid, 128, 0, st>>>(P, K, in, xn, out, out_split32, Hi, Wi, Ho, Wo);
+  stem_conv_kernel<CIN, COUT, S, SKIP><<<grid, 128, 0, st>>>(P, K, in, xn, out, out_split8, Hi, Wi, Ho, Wo);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }
@@ -248,8 +225,8 @@ __global__ void __launch_bounds__(128) stem01_kernel(const __grid_constant__ Ste
 }
 
 // xn (B,H,W) -> block1.1's split output (B,H/2,W/2,16) fp16 [hi8|lo8] through stem01_kernel.  H, W multiples of 4.
-static int launch_stem01(const float* hw, const LayerTable& t, const float* xn, __half* out_split8, int B, int H, int W,
-                         cudaStream_t st) {
+int launch_stem01(const float* hw, const LayerTable& t, const float* xn, __half* out_split8, int B, int H, int W,
+                  cudaStream_t st) {
   Stem01W P;
   memcpy(P.w0, hw + t.w_off[L_B1_0], sizeof(P.w0));
   memcpy(P.b0, hw + t.b_off[L_B1_0], sizeof(P.b0));
@@ -262,32 +239,23 @@ static int launch_stem01(const float* hw, const LayerTable& t, const float* xn, 
   return XF_OK;
 }
 
-static int g_stem_fused = 1;   // XFEAT_STEM_UNFUSED=1 in the environment selects the two-kernel path (A/B measurements)
-
-// xn (B,H,W) -> a1 (B,H,W,4) -> a2 (B,H/2,W/2,8) -> a3 (same,8) -> x1s (B,H/4,W/4,24) = block1(x) + skip1(x)
-// tc_tail != 0: only block1.0 and block1.1 run here (block1.1 writes split fp16 [hi8|lo8] into a2); block1.2 / block1.3 + skip
-// continue on the tensor cores (api.cu).
+// xn (B,H,W) -> a1 (B,H,W,4) -> a2 (B,H/2,W/2,8) -> a3 (same,8) -> x1s (B,H/4,W/4,24) = block1(x) + skip1(x), the fp32 schedule
 int launch_stem_chain(const float* h_weights, const LayerTable& t, const float* xn, float* a1, float* a2, float* a3,
-                      float* x1s, __half* x1s_split32, int B, int H, int W, cudaStream_t st, int tc_tail) {
+                      float* x1s, int B, int H, int W, cudaStream_t st) {
   const float* hw = h_weights;
-  int rc;
-  static const bool unfused = getenv("XFEAT_STEM_UNFUSED") != nullptr;
-  if (tc_tail && g_stem_fused && !unfused) return launch_stem01(hw, t, xn, (__half*)a2, B, H, W, st);
-  rc = launch_stem<1, 4, 1, false>(hw + t.w_off[L_B1_0], hw + t.b_off[L_B1_0], nullptr, nullptr, xn, nullptr, a1, nullptr, B, H, W, st);
+  int rc = launch_stem<1, 4, 1, false>(hw + t.w_off[L_B1_0], hw + t.b_off[L_B1_0], nullptr, nullptr, xn, nullptr, a1, nullptr, B, H, W, st);
   if (rc) return rc;
-  rc = launch_stem<4, 8, 2, false>(hw + t.w_off[L_B1_1], hw + t.b_off[L_B1_1], nullptr, nullptr, a1, nullptr, a2,
-                                   tc_tail ? (__half*)a2 : nullptr, B, H, W, st);
-  if (rc || tc_tail) return rc;
+  rc = launch_stem<4, 8, 2, false>(hw + t.w_off[L_B1_1], hw + t.b_off[L_B1_1], nullptr, nullptr, a1, nullptr, a2, nullptr, B, H, W, st);
+  if (rc) return rc;
   rc = launch_stem<8, 8, 1, false>(hw + t.w_off[L_B1_2], hw + t.b_off[L_B1_2], nullptr, nullptr, a2, nullptr, a3, nullptr, B, H / 2, W / 2, st);
   if (rc) return rc;
-  rc = launch_stem<8, 24, 2, true>(hw + t.w_off[L_B1_3], hw + t.b_off[L_B1_3], hw + t.w_off[L_SKIP1], hw + t.b_off[L_SKIP1],
-                                   a3, xn, x1s, x1s_split32, B, H / 2, W / 2, st);
-  return rc;
+  return launch_stem<8, 24, 2, true>(hw + t.w_off[L_B1_3], hw + t.b_off[L_B1_3], hw + t.w_off[L_SKIP1], hw + t.b_off[L_SKIP1],
+                                     a3, xn, x1s, nullptr, B, H / 2, W / 2, st);
 }
 
 }  // namespace xf
 
-// Test hook: block1.0 + block1.1 with block1.1's output split as xfeat_net hands it to block1.2 (conv impl 1 and 2).
+// Test hook: block1.0 + block1.1 with block1.1's output split as xfeat_net's tensor-core schedule hands it to block1.2.
 extern "C" int xfeat_debug_stem01(xfeat_ctx* ctx, int variant, const float* d_xn, int B, int H, int W, void* d_out_split,
                                   void* d_scratch, size_t scratch_bytes, void* stream) {
   XF_REQUIRE(ctx && d_xn && d_out_split && (variant == 0 || variant == 1) && B > 0 && B <= 65535 && H > 0 && W > 0 &&

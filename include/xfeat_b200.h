@@ -108,9 +108,10 @@ XF_API int xfeat_preprocess_scaled(const void* d_img, int dtype, int B, int C, i
                             int64_t stride_b, int64_t stride_c, int64_t stride_h, int64_t stride_w, int div255,
                             int H, int W, float scale_h, float scale_w, float* d_xn, double* d_stats, void* stream);
 
-/* Implementation switch of the conv layers inside xfeat_net (process-wide): 0 = fp32 CUDA-core kernels everywhere,
- * 1 = wgmma tensor-core kernels (split-fp16 operands, fp32 register accumulation), 2 = as 1 plus halo-patch operand
- * reuse for the 3x3 stride-1 layers.  xfeat_set_halo_desc_mode is a bring-up knob of mode 2 (1 = PTX base_offset rule). */
+/* Implementation switch of the conv layers inside xfeat_net (process-wide): 0 = fp32 CUDA-core kernels everywhere; any other
+ * value = the wgmma tensor-core schedule (split-fp16 operands, fp32 register accumulation, halo-patch operand reuse for the
+ * 3x3 stride-1 layers; the default), which xfeat_get_conv_impl reports as 2.  xfeat_set_halo_desc_mode is a bring-up knob of
+ * the halo-patch kernels (1 = PTX base_offset rule). */
 XF_API void xfeat_set_halo_desc_mode(int mode);
 XF_API void xfeat_set_conv_impl(int impl);
 XF_API int xfeat_get_conv_impl(void);
@@ -374,8 +375,9 @@ XF_API int xfeat_debug_conv_layer(xfeat_ctx* ctx, int layer, const float* d_in, 
 XF_API int xfeat_debug_conv_layer_tc(xfeat_ctx* ctx, int layer, const float* d_in, int B, int H, int W, float* d_out,
                                      void* d_scratch, size_t scratch_bytes, void* stream);
 
-/* Test hook: xfeat_debug_conv_layer_tc for any tensor-core layer, with the outputs the network passes on.  Follows
- * xfeat_set_conv_impl exactly as xfeat_net does.  d_in (B,H,W,Cin) fp32 NHWC is split into d_scratch (>= B*H*W*4*Cinp bytes,
+/* Test hook: xfeat_debug_conv_layer_tc for any tensor-core layer, with the outputs the network passes on.  Routes the layer as
+ * xfeat_net's tensor-core schedule does: the 3x3 stride-1 layers of 8, 24 and 64 channels on the halo-patch kernel, the others
+ * on the per-tap kernels.  d_in (B,H,W,Cin) fp32 NHWC is split into d_scratch (>= B*H*W*4*Cinp bytes,
  * Cinp = Cin rounded up to 8, 32, 64 or 128) first.  Outputs, at least one of them (Ho = H/stride, Wo = W/stride):
  *   d_out_f32 (B,Ho,Wo,Cout) fp32, or NULL;
  *   d_out_split (B,Ho,Wo,2*Cs) fp16 [hi(Cs) | lo(Cs)], Cs = 8 for block1.2, 32 for Cout = 24, else Cout; or NULL.
@@ -387,8 +389,8 @@ XF_API int xfeat_debug_conv_layer_tc_ex(xfeat_ctx* ctx, int layer, const float* 
 
 /* Test hook: block1.0 + block1.1 on the normalised gray image d_xn (B,H,W) fp32, H and W multiples of 4.  d_out_split
  * (B,H/2,W/2,16) fp16 [hi(8) | lo(8)] is block1.1's output split as block1.2 reads it.  variant 0 (the reference): block1.0
- * into d_scratch (>= B*H*W*16 bytes, its (B,H,W,4) fp32 output), then block1.1, one direct convolution each; 1: what xfeat_net
- * runs under conv impl 1 and 2, both layers in one kernel that recomputes block1.0 in registers (d_scratch unused). */
+ * into d_scratch (>= B*H*W*16 bytes, its (B,H,W,4) fp32 output), then block1.1, one direct convolution each; 1: what xfeat_net's
+ * tensor-core schedule runs, both layers in one kernel that recomputes block1.0 in registers (d_scratch unused). */
 XF_API int xfeat_debug_stem01(xfeat_ctx* ctx, int variant, const float* d_xn, int B, int H, int W, void* d_out_split,
                               void* d_scratch, size_t scratch_bytes, void* stream);
 

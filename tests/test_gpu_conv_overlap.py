@@ -26,7 +26,7 @@ def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def run_layer(xf, sd, layer, impl, B, Ho, Wo):
+def run_layer(xf, sd, layer, B, Ho, Wo):
     from accelerated_features_b200 import _lib, weights
     ks, stride, _, _ = sr.layer_geometry(layer)
     cout, cin = sd[weights.LAYERS[layer][0] + ".weight"].shape[:2]
@@ -39,15 +39,10 @@ def run_layer(xf, sd, layer, impl, B, Ho, Wo):
     out = torch.full((B, Ho, Wo, cout), float("nan"), device="cuda")
     split = torch.full((B, Ho, Wo, 2 * cs), float("nan"), dtype=torch.float16, device="cuda")
     scratch = torch.empty(B * H * W * 4 * cinp, dtype=torch.uint8, device="cuda")
-    old = xf._lib.xfeat_get_conv_impl()
-    xf._lib.xfeat_set_conv_impl(impl)
-    try:
-        _lib.check(xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out.data_ptr(), split.data_ptr(),
-                                                        None if skip is None else skip.data_ptr(), scratch.data_ptr(),
-                                                        scratch.numel(), torch.cuda.current_stream().cuda_stream), "conv_tc_ex")
-        torch.cuda.synchronize()
-    finally:
-        xf._lib.xfeat_set_conv_impl(old)
+    _lib.check(xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out.data_ptr(), split.data_ptr(),
+                                                    None if skip is None else skip.data_ptr(), scratch.data_ptr(),
+                                                    scratch.numel(), torch.cuda.current_stream().cuda_stream), "conv_tc_ex")
+    torch.cuda.synchronize()
     xc = x.permute(0, 3, 1, 2)
     ref = sr.reference(sd, layer, xc, skip)
     got = out.permute(0, 3, 1, 2)
@@ -63,21 +58,23 @@ def run_layer(xf, sd, layer, impl, B, Ho, Wo):
         assert bool((hi[..., cout:] == 0).all() and (lo[..., cout:] == 0).all()), "padded channels are not zero"
 
 
-# (layer, conv impl, name): the halo kernels (impl 2) and each conv_tc / conv_tc128 instantiation
+# (layer, kernel family, name): the halo kernels and each conv_tc / conv_tc128 instantiation; "3x3 64-ch per tap" is block4.0
+# (conv_tc_kernel<3,64,64>, stride 2)
 LAYERS = [
-    (5, 2, "halo 32-ch"), (8, 2, "halo 64-ch"), (9, 1, "1x1 64-ch"), (8, 1, "3x3 64-ch per tap"), (7, 2, "3x3 stride 2 32->64"),
-    (3, 2, "stem tail + skip1"), (13, 2, "block5.0 two N tiles"), (14, 2, "128-ch 3x3"), (16, 2, "128-ch 1x1"),
+    (5, "halo", "halo 32-ch"), (8, "halo", "halo 64-ch"), (9, "conv_tc", "1x1 64-ch"), (10, "conv_tc", "3x3 64-ch per tap"),
+    (7, "conv_tc", "3x3 stride 2 32->64"), (3, "conv_tc", "stem tail + skip1"), (13, "conv_tc", "block5.0 two N tiles"),
+    (14, "conv_tc", "128-ch 3x3"), (16, "conv_tc", "128-ch 1x1"),
 ]
 # output sizes of ONE tile per image: 4 x 8 fits the smallest halo tile (TW 8, TH 12), 8 x 16 one 128-pixel conv_tc tile
-ONE_TILE = {2: (4, 8), 1: (8, 16)}
+ONE_TILE = {"halo": (4, 8), "conv_tc": (8, 16)}
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", LAYERS, ids=lambda c: c[2].replace(" ", "_"))
 @pytest.mark.parametrize("edge", ["one_tile", "fewer_tiles_than_ctas", "waves_plus_one", "ragged"])
 def test_tile_count_edges(xf, oracle_state, sms, case, edge):
-    layer, impl, _ = case
-    ho, wo = ONE_TILE[impl if layer in (5, 8) else 1]
+    layer, family, _ = case
+    ho, wo = ONE_TILE[family]
     if edge == "one_tile":
         B = 1
     elif edge == "fewer_tiles_than_ctas":
@@ -86,7 +83,7 @@ def test_tile_count_edges(xf, oracle_state, sms, case, edge):
         B = 2 * sms + 1        # one tile per image: n_tiles = 2 * grid + 1, so the first CTA runs one tile more than the rest
     else:
         B, ho, wo = 5, 37, 53  # neither dimension a multiple of any tile shape
-    run_layer(xf, oracle_state, layer, impl, B, ho, wo)
+    run_layer(xf, oracle_state, layer, B, ho, wo)
 
 
 def test_build_logs_no_serialised_wgmma_or_epilogue_spills():

@@ -11,7 +11,7 @@ from tests import split_ref as sr
 from tests.test_gpu_conv_overlap import LAYERS, ONE_TILE
 
 MARGIN = 4096   # elements before and after each output (16-byte multiples for both dtypes)
-CASES = LAYERS + [(2, 2, "halo 8-ch")]
+CASES = LAYERS + [(2, "halo", "halo 8-ch")]
 
 
 @pytest.fixture(scope="module")
@@ -34,16 +34,11 @@ def geometry(sd, layer):
     return stride, cin, cout, cinp, cs
 
 
-def call(xf, layer, impl, x, B, H, W, out_ptr, split_ptr, skip, scratch):
-    old = xf._lib.xfeat_get_conv_impl()
-    xf._lib.xfeat_set_conv_impl(impl)
-    try:
-        rc = xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out_ptr, split_ptr,
-                                                   None if skip is None else skip.data_ptr(), scratch.data_ptr(), scratch.numel(),
-                                                   torch.cuda.current_stream().cuda_stream)
-        torch.cuda.synchronize()
-    finally:
-        xf._lib.xfeat_set_conv_impl(old)
+def call(xf, layer, x, B, H, W, out_ptr, split_ptr, skip, scratch):
+    rc = xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out_ptr, split_ptr,
+                                               None if skip is None else skip.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                                               torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
     return rc
 
 
@@ -61,8 +56,8 @@ def inputs(layer, B, Ho, Wo, stride, cin, cinp):
 @pytest.mark.parametrize("edge", ["one_tile", "fewer_tiles_than_ctas", "waves_plus_one", "ragged"])
 def test_outputs_stay_inside_their_tensors(xf, oracle_state, sms, case, edge):
     from accelerated_features_b200 import _lib
-    layer, impl, _ = case
-    ho, wo = ONE_TILE[impl if layer in (2, 5, 8) else 1]
+    layer, family, _ = case
+    ho, wo = ONE_TILE[family]
     B = {"one_tile": 1, "fewer_tiles_than_ctas": 3, "waves_plus_one": 2 * sms + 1, "ragged": 5}[edge]
     if edge == "ragged":
         ho, wo = 37, 53
@@ -72,7 +67,7 @@ def test_outputs_stay_inside_their_tensors(xf, oracle_state, sms, case, edge):
     out_buf = torch.full((n_out + 2 * MARGIN,), -12345.0, device="cuda")
     split_buf = torch.full((n_split + 2 * MARGIN,), -1234.0, dtype=torch.float16, device="cuda")
     out_keep, split_keep = out_buf.clone(), split_buf.clone()
-    _lib.check(call(xf, layer, impl, x, B, H, W, out_buf[MARGIN:].data_ptr(), split_buf[MARGIN:].data_ptr(), skip, scratch),
+    _lib.check(call(xf, layer, x, B, H, W, out_buf[MARGIN:].data_ptr(), split_buf[MARGIN:].data_ptr(), skip, scratch),
                "conv_tc_ex")
     for buf, keep, n, name in ((out_buf, out_keep, n_out, "fp32"), (split_buf, split_keep, n_split, "split")):
         assert torch.equal(buf[:MARGIN], keep[:MARGIN]), f"{name} output: write before the tensor"
@@ -80,16 +75,16 @@ def test_outputs_stay_inside_their_tensors(xf, oracle_state, sms, case, edge):
 
     out = torch.empty(B, ho, wo, cout, device="cuda")
     split = torch.empty(B, ho, wo, 2 * cs, dtype=torch.float16, device="cuda")
-    _lib.check(call(xf, layer, impl, x, B, H, W, out.data_ptr(), split.data_ptr(), skip, scratch), "conv_tc_ex")
+    _lib.check(call(xf, layer, x, B, H, W, out.data_ptr(), split.data_ptr(), skip, scratch), "conv_tc_ex")
     assert torch.equal(out_buf[MARGIN:MARGIN + n_out].view(torch.int32), out.reshape(-1).view(torch.int32))
     assert torch.equal(split_buf[MARGIN:MARGIN + n_split].view(torch.int16), split.reshape(-1).view(torch.int16))
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", [(8, 2, "halo"), (9, 1, "conv_tc"), (14, 2, "conv_tc128")], ids=lambda c: c[2])
+@pytest.mark.parametrize("case", [(8, "halo"), (9, "conv_tc"), (14, "conv_tc128")], ids=lambda c: c[1])
 @pytest.mark.parametrize("which", ["fp32", "split"])
 def test_misaligned_output_is_an_error(xf, oracle_state, case, which):
-    layer, impl, _ = case
+    layer, _ = case
     stride, cin, cout, cinp, cs = geometry(oracle_state, layer)
     B, ho, wo = 1, 8, 16
     H, W, x, skip, scratch = inputs(layer, B, ho, wo, stride, cin, cinp)
@@ -100,7 +95,7 @@ def test_misaligned_output_is_an_error(xf, oracle_state, case, which):
         out_ptr += 4
     else:
         split_ptr += 2
-    rc = call(xf, layer, impl, x, B, H, W, out_ptr, split_ptr, skip, scratch)
+    rc = call(xf, layer, x, B, H, W, out_ptr, split_ptr, skip, scratch)
     assert rc != 0
     assert "16-byte aligned" in xf._lib.xfeat_last_error().decode()
     assert bool((out == 0).all() and (split == 0).all()), "a refused call wrote its outputs"

@@ -142,7 +142,7 @@ def test_kernel_pairs_f32_refuses_other_impls(xf, table, impl):
     assert "does not take pre-split" in xf._lib.xfeat_last_error().decode()
 
 
-@pytest.mark.parametrize("conv", [1, 0])
+@pytest.mark.parametrize("conv", [2, 0])
 @pytest.mark.parametrize("fine_conf", [0.0, 0.25])
 def test_refine_pairs_equal_single_pair(xf, conv, fine_conf):
     g = torch.Generator().manual_seed(31)

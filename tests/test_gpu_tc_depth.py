@@ -48,26 +48,26 @@ def report(name, err, bound, model):
     assert err < bound, f"{name}: error {err:.3e} >= {bound:.1e}"
 
 
-# (layer, name, conv impl, B, H_in, W_in, tiles per CTA needed).  `need` = ring slots + 1 where the ring advances once per
-# tile (halo patch rings: 16 / 4 / 2 slots; 1x1 per-tap ring: 6 stages; stem tail: 4 stages of 9 taps), else 3.
+# (layer, name, B, H_in, W_in, tiles per CTA needed).  `need` = ring slots + 1 where the ring advances once per tile (halo patch
+# rings: 16 / 4 / 2 slots; 1x1 per-tap ring: 6 stages; stem tail: 4 stages of 9 taps), else 3.
 CONV_CASES = [
-    (2, "block1.2 halo 8-ch", 2, 6, 240, 320, 17),
-    (5, "block2.0 halo 32-ch", 2, 6, 120, 160, 5),
-    (8, "block3.1 halo 64-ch", 2, 12, 60, 80, 3),
-    (9, "block3.2 1x1 per-tap", 1, 32, 60, 80, 7),
-    (8, "block3.1 per-tap", 1, 12, 60, 80, 3),
-    (7, "block3.0 stride 2", 2, 12, 120, 160, 3),
-    (3, "block1.3 + skip1 stride 2", 2, 6, 240, 320, 5),
-    (13, "block5.0 two N tiles", 2, 180, 30, 40, 3),
-    (14, "block5.1 128-ch 3x3", 2, 26, 39, 52, 3),
-    (16, "block5.3 128-ch 1x1", 2, 26, 39, 52, 3),        # 52,728 pixels: the last tile is ragged
+    (2, "block1.2 halo 8-ch", 6, 240, 320, 17),
+    (5, "block2.0 halo 32-ch", 6, 120, 160, 5),
+    (8, "block3.1 halo 64-ch", 12, 60, 80, 3),
+    (9, "block3.2 1x1 per-tap", 32, 60, 80, 7),
+    (10, "block4.0 stride 2", 48, 60, 80, 3),
+    (7, "block3.0 stride 2", 12, 120, 160, 3),
+    (3, "block1.3 + skip1 stride 2", 6, 240, 320, 5),
+    (13, "block5.0 two N tiles", 180, 30, 40, 3),
+    (14, "block5.1 128-ch 3x3", 26, 39, 52, 3),
+    (16, "block5.3 128-ch 1x1", 26, 39, 52, 3),        # 52,728 pixels: the last tile is ragged
 ]
 
 
 @pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: c[1].replace(" ", "_"))
 def test_conv_layer_depth(xf, oracle_state, sms, case):
     from accelerated_features_b200 import _lib, weights
-    layer, name, impl, B, H, W, need = case
+    layer, name, B, H, W, need = case
     sd = oracle_state
     ks, stride, _, _ = sr.layer_geometry(layer)
     cout, cin = sd[weights.LAYERS[layer][0] + ".weight"].shape[:2]
@@ -83,10 +83,9 @@ def test_conv_layer_depth(xf, oracle_state, sms, case):
     out = torch.full((B, Ho, Wo, cout), float("nan"), device="cuda")
     split = torch.full((B, Ho, Wo, 2 * cs), float("nan"), dtype=torch.float16, device="cuda")
     scratch = torch.empty(B * H * W * 4 * cinp, dtype=torch.uint8, device="cuda")
-    with conv_impl(xf, impl):
-        _lib.check(xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out.data_ptr(), split.data_ptr(),
-                                                        None if skip is None else skip.data_ptr(), scratch.data_ptr(),
-                                                        scratch.numel(), torch.cuda.current_stream().cuda_stream), "conv_tc_ex")
+    _lib.check(xf._lib.xfeat_debug_conv_layer_tc_ex(xf._ctx, layer, x.data_ptr(), B, H, W, out.data_ptr(), split.data_ptr(),
+                                                    None if skip is None else skip.data_ptr(), scratch.data_ptr(),
+                                                    scratch.numel(), torch.cuda.current_stream().cuda_stream), "conv_tc_ex")
     torch.cuda.synchronize()
     xc = x.permute(0, 3, 1, 2)
     ref = sr.reference(sd, layer, xc, skip)
