@@ -70,6 +70,7 @@ SIGNATURES = {
     "xfeat_lg_match": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_f, c_i, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_lg_debug": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p, c_p, c_p, c_sz, c_p]),
     "xfeat_lg_debug_attention": (c_i, [c_p, c_p, c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p]),
+    "xfeat_lg_debug_assign": (c_i, [c_p, c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
     "xfeat_debug_conv_layer": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p]),
     "xfeat_debug_conv_layer_tc": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_sz, c_p]),
     "xfeat_debug_conv_layer_tc_ex": (c_i, [c_p, c_i, c_p, c_i, c_i, c_i, c_p, c_p, c_p, c_p, c_sz, c_p]),

@@ -843,3 +843,17 @@ extern "C" int xfeat_lg_debug_attention(const float* d_q, const float* d_k, cons
   lg::AttnArgs a{d_q, d_k, d_v, ld, d_n, n_max, groups, cross, d_out};
   return lg::attention(a, (cudaStream_t)stream);
 }
+
+extern "C" int xfeat_lg_debug_assign(const float* d_md, const float* d_lz, const int32_t* d_cnt, int batch, int n_max, float* d_lse,
+                                     float* d_best, int32_t* d_arg, void* stream) {
+  XF_REQUIRE(d_md && d_lz && d_cnt && d_lse && d_best && d_arg, "lg_debug_assign: null pointer");
+  XF_REQUIRE(batch > 0 && n_max > 0 && (size_t)2 * batch * n_max <= 0x7fffffffu, "lg_debug_assign: bad shape");
+  cudaStream_t st = (cudaStream_t)stream;
+  XF_DYN_SMEM(lg::lg_assign_kernel, lg::assign_smem());
+  for (int pass = 0; pass < 2; ++pass) {
+    lg::AssignArgs a{d_md, d_lz, d_cnt, n_max, batch, d_lse, d_best, d_arg, pass};
+    lg::lg_assign_kernel<<<dim3(cdiv(n_max, lg::BM), batch, 2), 256, lg::assign_smem(), st>>>(a);
+    XF_LAUNCH_CHECK();
+  }
+  return XF_OK;
+}

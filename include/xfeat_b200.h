@@ -366,6 +366,13 @@ XF_API int xfeat_lg_debug(xfeat_lg_ctx* ctx, int batch, int n_max, const float* 
 XF_API int xfeat_lg_debug_attention(const float* d_q, const float* d_k, const float* d_v, int ld, const int32_t* d_n, int groups,
                                     int n_max, int cross, float* d_out, void* stream);
 
+/* Test hook: LighterGlue's assignment alone.  d_md (2*batch, n_max, 96) fp32 rows (final_proj(x) / 96^0.25; group b is image 0
+ * of pair b, group batch + b its image 1), d_lz (2*batch, n_max) logsigmoid(matchability), d_cnt (2*batch) int32 counts.
+ * For the rows below each count: d_lse = log-sum-exp of S = md0 md1^T along the row (group b) or column (group batch + b), and
+ * d_best / d_arg = maximum / first arg-maximum of (S - lse0) + (S - lse1) + (lz0 + lz1) along it. */
+XF_API int xfeat_lg_debug_assign(const float* d_md, const float* d_lz, const int32_t* d_cnt, int batch, int n_max, float* d_lse,
+                                 float* d_best, int32_t* d_arg, void* stream);
+
 /* Test hook: run one folded conv layer of the packed table (index into csrc/layers.h) through the generic
  * kernels. in (B,Hi,Wi,Cin) NHWC -> out (B,Ho,Wo,Cout). */
 XF_API int xfeat_debug_conv_layer(xfeat_ctx* ctx, int layer, const float* d_in, int B, int Hi, int Wi, float* d_out,

@@ -116,8 +116,8 @@ def match(sd, kpts0, desc0, size0, kpts1, desc1, size1, min_conf: float = 0.1, p
           n_layers: int = N_LAYERS) -> Dict[str, object]:
     """One pair.  Returns idx0 (ascending), idx1, scores (float of `dtype`), and the diagnostics the parity tests use:
     'x' (the two final descriptor sets), 'ind' (surviving original indices per image), 'keep' (per pruned layer, per image: the
-    keep mask or None), 'z' (matchability logits at each pruning step), 'row_max' / 'row_gap' / 'col_gap' (assignment row
-    maximum and top-2 gaps over the surviving points), 'mscore' (exp(row max)) and the mutual mask.  `n_layers` < 6 stops after
+    keep mask or None), 'z' (matchability logits at each pruning step), 'row_max' / 'col_max' / 'row_gap' / 'col_gap' (assignment row
+    and column maxima and top-2 gaps over the surviving points), 'mscore' (exp(row max)) and the mutual mask.  `n_layers` < 6 stops after
     that many layers and returns only 'x', 'ind', 'keep' and 'z'."""
     dt = np.dtype(dtype).type
     m = _Model(sd, dt)
@@ -180,5 +180,6 @@ def match(sd, kpts0, desc0, size0, kpts1, desc1, size1, min_conf: float = 0.1, p
         t = -np.partition(-a, 1, axis=axis)
         return (t.take(0, axis) - t.take(1, axis))
     out.update(idx0=inds[0][i0].astype(np.int64), idx1=inds[1][m0[i0]].astype(np.int64), scores=mscore[i0].astype(dt),
-               row_max=rmax, row_arg=m0, col_arg=m1, row_gap=gap(sc, 1), col_gap=gap(sc, 0), mscore=mscore, mutual=mutual)
+               row_max=rmax, row_arg=m0, col_max=sc.max(0), col_arg=m1, row_gap=gap(sc, 1), col_gap=gap(sc, 0), mscore=mscore,
+               mutual=mutual)
     return out
