@@ -60,7 +60,8 @@ __device__ __forceinline__ bool nms_is_max(const float* __restrict__ hb, int H, 
     for (int dx = -r; dx <= r; ++dx) {
       const int xx = x + dx;
       if (xx < 0 || xx >= W) continue;
-      if (__ldg(hb + (int64_t)yy * W + xx) > v) return false;
+      // !(nb <= v), not nb > v: a NaN neighbour suppresses the pixel, as NaN propagates through the reference's max_pool2d
+      if (!(__ldg(hb + (int64_t)yy * W + xx) <= v)) return false;
     }
   }
   return true;
@@ -256,7 +257,9 @@ extern "C" int xfeat_nms_count(const float* d_heat, int B, int H, int W, int ker
 
 extern "C" int xfeat_nms_write(const float* d_heat, int B, int H, int W, int kernel_size, float threshold, int64_t* d_pos,
                                int pos_cap, void* d_ws, size_t ws_bytes, void* stream) {
-  XF_REQUIRE(d_heat && d_pos && d_ws && B > 0 && B <= 65535 && H > 0 && W > 0 && pos_cap >= 0, "nms_write: bad arguments");
+  // pos_cap 0 (every image empty) writes nothing: d_pos may then be the null pointer of an empty (B, 0, 2) tensor
+  XF_REQUIRE(d_heat && (d_pos || pos_cap == 0) && d_ws && B > 0 && B <= 65535 && H > 0 && W > 0 && pos_cap >= 0,
+             "nms_write: bad arguments");
   XF_REQUIRE(kernel_size >= 1 && (kernel_size & 1), "nms: kernel_size must be odd (got %d)", kernel_size);
   XF_REQUIRE(ws_bytes >= xfeat_nms_workspace_bytes(B, H, W), "nms_write: workspace too small");
   if (pos_cap == 0) return XF_OK;
@@ -270,7 +273,7 @@ extern "C" int xfeat_nms_write(const float* d_heat, int B, int H, int W, int ker
 }
 
 extern "C" int xfeat_subpix_softmax2d(const float* d_maps, int64_t n, float temp, float* d_out, void* stream) {
-  XF_REQUIRE(d_maps && d_out && n >= 0, "subpix_softmax2d: bad arguments");
+  XF_REQUIRE(n >= 0 && (n == 0 || (d_maps && d_out)), "subpix_softmax2d: bad arguments");   // n = 0: empty tensors, null
   if (n == 0) return XF_OK;
   xf::subpix_softmax2d_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_maps, n, temp, d_out);
   XF_LAUNCH_CHECK();
@@ -301,8 +304,8 @@ extern "C" int xfeat_fine_matcher(xfeat_ctx* ctx, const float* d_x, int n, float
 
 extern "C" int xfeat_interpolate_sparse(const float* d_x, const float* d_pos, int B, int C, int Hm, int Wm, int N, int H, int W,
                                         int mode, float* d_out, void* stream) {
-  XF_REQUIRE(d_x && d_pos && d_out && B > 0 && C > 0 && Hm > 0 && Wm > 0 && N >= 0 && mode >= 0 && mode <= 2,
-             "interpolate_sparse: bad arguments");
+  XF_REQUIRE(d_x && (N == 0 || (d_pos && d_out)) && B > 0 && C > 0 && Hm > 0 && Wm > 0 && N >= 0 && mode >= 0 && mode <= 2,
+             "interpolate_sparse: bad arguments");   // N = 0: pos and out are empty tensors, null
   const int64_t total = (int64_t)B * N * C;
   if (total == 0) return XF_OK;
   xf::interpolate_sparse_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_x, d_pos, C, Hm, Wm, N, H, W,

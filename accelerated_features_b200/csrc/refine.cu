@@ -140,7 +140,8 @@ __global__ void __launch_bounds__(1024) refine_compact_kernel(const float* __res
     if (threadIdx.x == 0) s_base = base + total;
     __syncthreads();
   }
-  if (threadIdx.x == 0) n_refined[pair] = s_base;
+  // a negative count (XF_N_OVERFLOW from the matcher) is a status, not "no matches": pass it through
+  if (threadIdx.x == 0) n_refined[pair] = n_matches[pair] < 0 ? n_matches[pair] : s_base;
 }
 
 struct RefineWs {

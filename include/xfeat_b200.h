@@ -236,7 +236,8 @@ XF_API size_t xfeat_refine_workspace_bytes(int batch, int n_max);
  * keypoints d_kpts0 (batch,n_max,2) / d_kpts1 (batch,n1_max,2), d_scales0 (batch,n_max), coarse matches d_idx0/d_idx1
  * (batch,n_max) + d_n_matches (the two image sets may yield different numbers of coarse features, as reference batch_match
  * allows).  Output d_matches (batch,n_max,4) = (x0+dx*s, y0+dy*s, x1, y1) for rows with conf > fine_conf, order preserved;
- * d_n_refined (batch). */
+ * d_n_refined (batch).  Counts above n_max are clamped to n_max; a negative count (XF_N_OVERFLOW) is passed through to
+ * d_n_refined for that pair, which refines nothing.  Rows of d_matches past d_n_refined[p] are not written. */
 XF_API int xfeat_refine(xfeat_ctx* ctx, const float* d_desc0, const float* d_desc1, const float* d_kpts0,
                  const float* d_kpts1, const float* d_scales0, const int64_t* d_idx0, const int64_t* d_idx1,
                  const int32_t* d_n_matches, int batch, int n_max, int n1_max, float fine_conf, float* d_matches,
@@ -262,7 +263,9 @@ XF_API int xfeat_kpts_heatmap(const float* d_logits, int B, int Hc, int Wc, floa
 /* replaces: XFeat.NMS (xfeat.py:249-263): pos = (x == MaxPool2d(kernel_size, stride 1, pad kernel_size/2)(x)) & (x > threshold),
  * positions (x, y) int64 in raster order.  Two calls, as the reference's own nonzero() needs the count on the host:
  * xfeat_nms_count fills d_counts (B) int32; the caller sizes d_pos (B, pos_cap, 2) (zero-initialised = the reference's
- * padding, pos_cap = max count) and xfeat_nms_write fills it.  d_ws: xfeat_nms_workspace_bytes, kept between the calls. */
+ * padding, pos_cap = max count) and xfeat_nms_write fills it.  d_ws: xfeat_nms_workspace_bytes, kept between the calls.
+ * A NaN pixel suppresses every pixel in its window and is never kept (NaN propagates through MaxPool2d).  Calls with nothing
+ * to write (pos_cap = 0 here, n = 0 / N = 0 below) accept null output and position pointers, as empty tensors have. */
 XF_API size_t xfeat_nms_workspace_bytes(int B, int H, int W);
 XF_API int xfeat_nms_count(const float* d_heat, int B, int H, int W, int kernel_size, float threshold, int32_t* d_counts,
                            void* d_ws, size_t ws_bytes, void* stream);
@@ -280,7 +283,11 @@ XF_API int xfeat_interpolate_sparse(const float* d_x, const float* d_pos, int B,
 XF_API int xfeat_subpix_softmax2d(const float* d_maps, int64_t n, float temp, float* d_out, void* stream);
 
 /* replaces: XFeatModel.fine_matcher (model.py:97-111; Linear + BatchNorm1d(affine=False) folded + ReLU x4, Linear):
- * d_x (n,128) -> d_out (n,64) logits. */
+ * d_x (n,128) -> d_out (n,64) logits.  Domain of the tensor-core schedule (the default): max |x| <= 2^13.  There the logits
+ * are finite and within 6e-4 x max(1, max|x| / 8.3) of float64 (the split error is relative, so it grows with the
+ * activations; coarse descriptors have max |x| ~ 8).  Inputs are neither refused nor rescaled: above 65504 the unscaled fp16
+ * split of the input overflows, and at max |x| ~ 2.5e5 the logits are finite but wrong by their own magnitude.  The fp32
+ * schedule (xfeat_set_conv_impl(0)) has no such limit. */
 XF_API size_t xfeat_fine_matcher_workspace_bytes(int n);
 XF_API int xfeat_fine_matcher(xfeat_ctx* ctx, const float* d_x, int n, float* d_out, void* d_ws, size_t ws_bytes, void* stream);
 
