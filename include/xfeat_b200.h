@@ -162,10 +162,10 @@ XF_API int xfeat_detect_dense(xfeat_ctx* ctx, const float* d_feats, const float*
                        void* stream);
 
 /* Implementation switch of xfeat_mnn_match (process-wide): 0 = fp32 CUDA-core kernel; 1 = wgmma tensor-core kernel
- * (split-fp16 operands, fp32 register accumulation, one three-term GEMM per direction; default); 2 = wgmma, single GEMM with the
- * column arg-max reduced in the epilogue; 3 = implementation 1, one CTA per work item; 4 = filter +
- * exact re-score: one fp16 pass per direction tracking top-1 / top-2, then implementation 1's kernel only on the rows whose
- * gap is within the rounding bound of the dropped split terms.  All honour the same tie rule; 1-4 return identical results.
+ * (split-fp16 operands, fp32 register accumulation, one three-term GEMM per pair whose tiles give both the row and the column
+ * arg-max; default); 2 = wgmma, persistent, one three-term GEMM per direction; 3 = implementation 2 with one CTA per work item;
+ * 4 = filter + exact re-score: one fp16 pass per direction tracking top-1 / top-2, then implementation 3's kernel only on the
+ * rows whose gap is within the rounding bound of the dropped split terms.  All honour the same tie rule; 1-4 return identical results.
  * Values outside 0..4 are clamped. */
 XF_API void xfeat_set_mnn_impl(int impl);
 XF_API int xfeat_get_mnn_impl(void);
@@ -192,7 +192,7 @@ XF_API int xfeat_mnn_match_bounded(const float* d_f1, const int32_t* d_n1, int n
                             int32_t* d_n_matches, void* d_ws, size_t ws_bytes, void* stream);
 
 /* xfeat_mnn_match on operands the producer already split (xfeat_detect_sparse_split): d_f1s / d_f2s (batch, n_pad, 128) fp16 rows
- * [hi(64) | lo(64)] of descriptor * 2^scale_log2.  Same outputs and tie rule as xfeat_mnn_match; implementations 1 and 3 only
+ * [hi(64) | lo(64)] of descriptor * 2^scale_log2.  Same outputs and tie rule as xfeat_mnn_match; implementations 1-3 only
  * (XF_E_UNSUPPORTED otherwise). */
 XF_API size_t xfeat_mnn_presplit_workspace_bytes(int batch, int n1_max, int n2_max);
 XF_API int xfeat_mnn_match_presplit(const void* d_f1s, const int32_t* d_n1, int n1_max, const void* d_f2s, const int32_t* d_n2,

@@ -67,7 +67,7 @@ def run(xf, f1, f2, thr):
     return i0.cpu().numpy(), i1.cpu().numpy()
 
 
-TC_IMPLS = [4, 1, 2, 3]   # 4: filter + exact re-score (default), 1: one 3-term GEMM per direction, 2: single GEMM (row + column arg-max), 3: 1 with one CTA per work item
+TC_IMPLS = [4, 1, 2, 3]   # 1: single 3-term GEMM giving the row and column arg-max (default), 2: one 3-term GEMM per direction, 3: 2 with one CTA per work item, 4: filter + exact re-score
 
 
 @pytest.mark.parametrize("impl", TC_IMPLS)
