@@ -381,100 +381,141 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist2_kernel(const __
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Default kernel (implementation 1): S = F1.F2^T is computed ONCE per pair, in the three-term order of mnn_tile_mma(dir = 0),
-// and the same accumulator tile yields both arg-maxes.  Persistent CTAs walk items (pair, 256-row block of set 1); an item
-// streams every 128-column B tile of set 2.
+// and the same accumulator tile yields both arg-maxes.  Persistent CTAs walk items (pair, 256-column block of set 2), pair-major
+// so that the CTAs in flight share one pair's set 1 in L2.  The item's two 128-column slabs of set 2 (the B operand) stay
+// resident and TMA streams every 128-row A tile of set 1 past them; warpgroup w owns slab w for the whole item.
 //
-// Ping-pong: the two consumer warpgroups (one 128-row slab each) take turns issuing their MMAs on a B tile (named barriers 1
-// and 2 pass the turn), so warpgroup 0 reduces tile t while the tensor pipe runs warpgroup 1's MMAs on t, and warpgroup 1
-// reduces t while warpgroup 0's MMAs on t+1 run.  A B stage is released once all eight consumer warps' MMAs on it retired.
+// Ping-pong: the two consumer warpgroups take turns issuing their MMAs on an A tile (named barriers 1 and 2 pass the turn), so
+// warpgroup 0 reduces tile t while the tensor pipe runs warpgroup 1's MMAs on t, and warpgroup 1 reduces t while warpgroup 0's
+// MMAs on t+1 run.  Each warpgroup commits a tile's MMAs as two groups (rows 0-63, rows 64-127) and starts the epilogue of the
+// first half while the tensor cores still run the second.  An A stage is released once all eight consumer warps' MMAs on it
+// retired.
 //
-// Epilogue of one slab tile, per thread 4 rows x 32 columns:
-//   rows:    value-only running maximum (fmaxf over the thread's columns, then the quad of lanes that shares the row); the
-//            column index is looked up -- first equal column, ascending -- only for rows whose tile maximum beats the running
-//            best (strictly: an earlier tile keeps a tie).
-//   columns: first maximum over the thread's rows r, r+8, r+64, r+72 (ascending, strict >), fp32 maximum across the 8 row
-//            lanes, then the lowest row that holds it (integer minimum over the lanes that match); the four warps' (value,
-//            row) partials meet in shared memory behind a 128-thread barrier, and one red.global.max.u64 per column and slab
-//            merges them into best21 as packed (value, ~row) -- the format and tie rule of a row arg-max of S21, which
-//            mnn_finalize_kernel reads.  The packed max is associative and commutative: the atomic order does not matter.
-// Columns past n2 (last tile) and rows past n1 (last row block) are set to -inf before the reductions.
+// Epilogue of one tile, per thread 4 rows x 32 columns (mnn_half_epilogue, once per 64-row half):
+//   rows:    maximum of each row over the slab's 128 columns (fp32 maximum over the thread's columns, then the quad of lanes
+//            that shares the row) and the first column that holds it; one red.global.max.u64 per row, slab and item merges
+//            the packed (value, ~column) into best12.  The packed max is associative and commutative, so the atomic order
+//            does not matter and the lowest column wins ties (torch's first-index rule).
+//   columns: a running (value, row) per column over all tiles of the item, strict > in ascending row order (tiles ascend,
+//            and h = 0..3 is r, r+8, r+64, r+72), so each thread keeps its first row on ties.  Nothing crosses lanes.
+// Once per item, the 8 row lanes (shuffles) and the 4 warps (shared memory) combine the column partials as packed (value,
+// ~row) maxima.  A column lives in one slab of one item, so best21 is written once, without atomics, in the format and tie
+// rule of a row arg-max of S21 that mnn_finalize_kernel reads.
+// Rows past n1 (last tile) and columns past n2 (last item) are set to -inf before the reductions.
 //
-// Shared memory: A double buffered across items (2 x 64 KB), a 2-stage B ring (2 x 32 KB), the column partials
-// [slab][tile parity][warp][column] (float value, int row) = 16 KB.  A third B stage does not fit beside the partials
-// (227 KB per block); with both directions in one item the ring only has to cover the load of tile t+2 during the two
-// slabs' MMAs on tile t+1.
+// Shared memory: the B slabs double buffered across items (2 x 64 KB), a 2-stage A ring (2 x 32 KB), the column partials
+// [slab][item parity][warp][column] as packed u64 = 16 KB.  A third A stage does not fit beside them (227 KB per block).
+// Registers: the accumulator (128) and the column state (64) need more than the 168 per thread that 384 threads leave, so the
+// producer is a whole warpgroup (warps 8-11; one lane of warp 8 issues the loads) that hands its registers to the consumers
+// with setmaxnreg (40 / 232).
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int TCF_NSB = 2;
-constexpr size_t TCF_COL_BYTES = 2 * 2 * 4 * 128 * sizeof(float2);
-constexpr size_t TCF_SMEM = 1024 + (size_t)(8 + 2 * TCF_NSB) * TC_BOX_BYTES + 256 + TCF_COL_BYTES;
+constexpr int TCF_THREADS = 384;
+constexpr int TCF_NSA = 2;
+constexpr size_t TCF_COL_BYTES = 2 * 2 * 4 * 128 * sizeof(unsigned long long);
+constexpr size_t TCF_SMEM = 1024 + (size_t)(8 + 2 * TCF_NSA) * TC_BOX_BYTES + 256 + TCF_COL_BYTES;
 
 __device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// fragment element (h, j, e) as an lvalue (see tc::frag_val)
-__device__ __forceinline__ float& frag_ref(float (&d0)[64], float (&d1)[64], int h, int j, int e) {
-  return (h < 2) ? d0[4 * j + 2 * h + e] : d1[4 * j + 2 * (h - 2) + e];
-}
-
-// running row maximum of the thread's four rows: bv = value, bc = column (first index on ties)
-__device__ __forceinline__ void mnn_row_update(const float (&acc0)[64], const float (&acc1)[64], int col0, int lane,
-                                               float (&bv)[4], int (&bc)[4]) {
-  const int cq = 2 * (lane & 3);
+// mnn_tile_mma_issue(dir = 0) as two commit groups, rows 0-63 of the A tile (acc0) and then rows 64-127 (acc1), so that
+// wgmma_wait<1> hands acc0 to the epilogue while the tensor cores still run acc1.  Every accumulator adds the same products in
+// the same order as mnn_tile_mma_issue.
+__device__ __forceinline__ void mnn_tile_mma_issue_halves(float (&acc0)[64], float (&acc1)[64], uint32_t a_tile, uint32_t b_slab) {
+  tc::wgmma_fence();
 #pragma unroll
-  for (int h = 0; h < 4; ++h) {
-    float m[8];
+  for (int half = 0; half < 2; ++half) {
 #pragma unroll
-    for (int q = 0; q < 8; ++q)
-      m[q] = fmaxf(fmaxf(tc::frag_val(acc0, acc1, h, 2 * q, 0), tc::frag_val(acc0, acc1, h, 2 * q, 1)),
-                   fmaxf(tc::frag_val(acc0, acc1, h, 2 * q + 1, 0), tc::frag_val(acc0, acc1, h, 2 * q + 1, 1)));
-    float mx = fmaxf(fmaxf(fmaxf(m[0], m[1]), fmaxf(m[2], m[3])), fmaxf(fmaxf(m[4], m[5]), fmaxf(m[6], m[7])));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-    const bool upd = mx > bv[h];
-    if (__any_sync(0xffffffffu, upd)) {
-      int c = 1 << 30;
+    for (int kb = 0; kb < 3; ++kb) {
+      const uint64_t da = tc::make_desc_sw128(a_tile + (kb == 2 ? 1 : 0) * TC_BOX_BYTES, 1024) + half * MT_HALF;
+      const uint64_t db = tc::make_desc_sw128(b_slab + (kb == 1 ? 1 : 0) * TC_BOX_BYTES, 1024);
 #pragma unroll
-      for (int j = 15; j >= 0; --j)
-#pragma unroll
-        for (int e = 1; e >= 0; --e) c = (tc::frag_val(acc0, acc1, h, j, e) == mx) ? 8 * j + e : c;
-      c += cq;
-      c = min(c, __shfl_xor_sync(0xffffffffu, c, 1));
-      c = min(c, __shfl_xor_sync(0xffffffffu, c, 2));
-      if (upd) {
-        bv[h] = mx;
-        bc[h] = col0 + c;
-      }
+      for (int k = 0; k < 4; ++k) tc::wgmma_f16<128>(half ? acc1 : acc0, da + 2 * k, db + 2 * k, (kb | k) ? 1u : 0u);
     }
+    tc::wgmma_commit();
   }
 }
 
-// column maxima of one tile over the warp's 32 rows of the slab: sc[column] = (value, row within the slab of its first row)
-__device__ __forceinline__ void mnn_col_warp(const float (&acc0)[64], const float (&acc1)[64], int wt, float2* sc) {
-  const int lane = wt & 31, cq = 2 * (lane & 3);
-  const int r0 = 16 * (wt >> 5) + (lane >> 2);   // row of h = 0; h = 1..3 are r0 + 8, r0 + 64, r0 + 72
+// Epilogue of one 64-row half d of a slab tile (d = acc0: fragment rows h = 0, 1; d = acc1: h = 2, 3, as tc::frag_val): element
+// (h, j, e) of the half is d[4j + 2h + e], row row[H0 + h] of the pair, column col0 + 8j + 2(lane%4) + e of set 2.
+//   Masking: columns from n_valid on and, in a tile that reaches past n1 (rows_partial), rows from n_rows on become -inf.
+//   Rows: the maximum over the slab's 128 columns (thread, then the quad of lanes that shares the row) and the first column
+//     that holds it, merged into best12 with red.global.max (a row that is all -inf writes nothing).  Both rows go through
+//     each step together and the first-column search runs as four short select chains per row, which keeps independent work
+//     in flight: while the tensor cores run MMAs, each scheduler has one warp in this epilogue.
+//   Columns: the running (value, row) of column 8j + 2(lane%4) + e is (cv, cr)[2j + e], updated with strict > in ascending row
+//     order (H0 = 0 before H0 = 2, tiles ascending), so each thread keeps its first row on ties.
+template <int H0>
+__device__ __forceinline__ void mnn_half_epilogue(float (&d)[64], const int (&row)[4], int col0, int n_valid, int n_rows,
+                                                  bool rows_partial, int lane, unsigned long long* best12, float (&cv)[32], int (&cr)[32]) {
+  const int cq = 2 * (lane & 3);
+  if (n_valid < TC_BN) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        if (8 * j + cq + e >= n_valid) d[4 * j + e] = d[4 * j + 2 + e] = -INFINITY;
+  }
+  if (rows_partial)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (row[H0 + h] >= n_rows)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d[4 * (i >> 1) + 2 * h + (i & 1)] = -INFINITY;
+
+  float mx[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float m[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      m[q] = fmaxf(fmaxf(d[8 * q + 2 * h], d[8 * q + 2 * h + 1]), fmaxf(d[8 * q + 4 + 2 * h], d[8 * q + 5 + 2 * h]));
+    mx[h] = fmaxf(fmaxf(fmaxf(m[0], m[1]), fmaxf(m[2], m[3])), fmaxf(fmaxf(m[4], m[5]), fmaxf(m[6], m[7])));
+  }
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], o));
+  int c[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    int cs[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {   // columns 32g .. 32g+31 of the tile, first equal one
+      cs[g] = 1 << 30;
+#pragma unroll
+      for (int j = 4 * g + 3; j >= 4 * g; --j)
+#pragma unroll
+        for (int e = 1; e >= 0; --e) cs[g] = (d[4 * j + 2 * h + e] == mx[h]) ? 8 * j + e : cs[g];
+    }
+    c[h] = min(min(cs[0], cs[1]), min(cs[2], cs[3])) + cq;
+  }
+#pragma unroll
+  for (int o = 1; o < 4; o <<= 1)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) c[h] = min(c[h], __shfl_xor_sync(0xffffffffu, c[h], o));
+
 #pragma unroll
   for (int j = 0; j < 16; ++j)
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      float m = tc::frag_val(acc0, acc1, 0, j, e);
-      int k = 0;
-      const float v1 = tc::frag_val(acc0, acc1, 1, j, e), v2 = tc::frag_val(acc0, acc1, 2, j, e),
-                  v3 = tc::frag_val(acc0, acc1, 3, j, e);
-      if (v1 > m) { m = v1; k = 8; }
-      if (v2 > m) { m = v2; k = 64; }
-      if (v3 > m) { m = v3; k = 72; }
-      float mx = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 8));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 16));
-      int r = (m == mx) ? r0 + k : 1 << 30;
-      r = min(r, __shfl_xor_sync(0xffffffffu, r, 4));
-      r = min(r, __shfl_xor_sync(0xffffffffu, r, 8));
-      r = min(r, __shfl_xor_sync(0xffffffffu, r, 16));
-      if (lane < 4) sc[8 * j + cq + e] = make_float2(mx, __int_as_float(r));
+      const float v0 = d[4 * j + e], v1 = d[4 * j + 2 + e];
+      const float m = v1 > v0 ? v1 : v0;
+      const int r = v1 > v0 ? row[H0 + 1] : row[H0];
+      if (m > cv[2 * j + e]) { cv[2 * j + e] = m; cr[2 * j + e] = r; }
     }
+
+  if ((lane & 3) == 0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (mx[h] != -INFINITY) atomicMax(best12 + row[H0 + h], pack_vi(mx[h], (uint32_t)(col0 + c[h])));
+  }
 }
 
-__global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
+__global__ void __launch_bounds__(TCF_THREADS, 1) mnn_tc_persist_kernel(const __grid_constant__ TcMaps maps,
                                                                        const int* __restrict__ n1p, int n1_max,
                                                                        const int* __restrict__ n2p, int n2_max, int n_pad, int batch,
                                                                        unsigned long long* __restrict__ best12,
@@ -482,69 +523,71 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
                                                                        const int2* __restrict__ pairs) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* base = reinterpret_cast<unsigned char*>(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  unsigned char* sA = base;                       // [buffer 2][slab 2][hi, lo] boxes
-  unsigned char* sB = base + 8 * TC_BOX_BYTES;    // [stage TCF_NSB][hi, lo] boxes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (8 + 2 * TCF_NSB) * TC_BOX_BYTES);
-  uint64_t* a_full = bars;                        // [2]
-  uint64_t* a_empty = bars + 2;                   // [2]
-  uint64_t* b_full = bars + 4;                    // [TCF_NSB]
-  uint64_t* b_empty = b_full + TCF_NSB;           // [TCF_NSB]
-  float2* sCol = reinterpret_cast<float2*>(base + (8 + 2 * TCF_NSB) * TC_BOX_BYTES + 256);   // [slab 2][parity 2][warp 4][128]
+  unsigned char* sB = base;                       // [buffer 2][slab 2][hi, lo] boxes
+  unsigned char* sA = base + 8 * TC_BOX_BYTES;    // [stage TCF_NSA][hi, lo] boxes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + (8 + 2 * TCF_NSA) * TC_BOX_BYTES);
+  uint64_t* b_full = bars;                        // [2]
+  uint64_t* b_empty = bars + 2;                   // [2]
+  uint64_t* a_full = bars + 4;                    // [TCF_NSA]
+  uint64_t* a_empty = a_full + TCF_NSA;           // [TCF_NSA]
+  unsigned long long* sCol =
+      reinterpret_cast<unsigned long long*>(base + (8 + 2 * TCF_NSA) * TC_BOX_BYTES + 256);   // [slab 2][parity 2][warp 4][128]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int RB = n_pad / TC_ROWS;
-  const int n_items = batch * RB;
+  const int CB = n_pad / TC_ROWS;   // 256-column blocks per pair
+  const int n_items = batch * CB;
 
   if (warp == 8 && lane == 0) {
     tc::tma_prefetch_desc(&maps.m1);
     tc::tma_prefetch_desc(&maps.m2);
     for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&a_full[i], 1);
-      tc::mbar_init(&a_empty[i], 8);
-    }
-    for (int i = 0; i < TCF_NSB; ++i) {
       tc::mbar_init(&b_full[i], 1);
       tc::mbar_init(&b_empty[i], 8);
+    }
+    for (int i = 0; i < TCF_NSA; ++i) {
+      tc::mbar_init(&a_full[i], 1);
+      tc::mbar_init(&a_empty[i], 8);
     }
     tc::fence_barrier_init();
   }
   __syncthreads();
 
-  // item -> (pair, row block) and the images (ia, ib) of its A and B rows (pairs: see mnn_tc_kernel); every role walks the same
-  // sequence and skips the same (empty) items
-  auto decode = [&](int item, int& pair, int& row0, int& n_rows, int& n_cols, int& ia, int& ib) {
-    pair = item / RB;
-    row0 = (item - pair * RB) * TC_ROWS;
+  // item -> (pair, column block) and the images (ia, ib) of its A and B rows (pairs: see mnn_tc_kernel); every role walks the
+  // same sequence and skips the same (empty) items
+  auto decode = [&](int item, int& pair, int& col0, int& n_rows, int& n_cols, int& ia, int& ib) {
+    pair = item / CB;
+    col0 = (item - pair * CB) * TC_ROWS;
     const int2 ij = pairs ? __ldg(pairs + pair) : make_int2(pair, pair);
     ia = ij.x;
     ib = ij.y;
     n_rows = n1p ? min(__ldg(n1p + ia), n1_max) : n1_max;
     n_cols = n2p ? min(__ldg(n2p + ib), n2_max) : n2_max;
-    return row0 < n_rows && n_cols > 0;
+    return col0 < n_cols && n_rows > 0;
   };
 
-  if (warp == 8) {
-    if (tc::elect_one()) {
-      uint32_t ai = 0, bi = 0;
+  if (warp >= 8) {
+    setmaxnreg_dec<40>();
+    if (warp == 8 && tc::elect_one()) {
+      uint32_t bi = 0, ai = 0;
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        int pair, row0, n_rows, n_cols, ia, ib;
-        if (!decode(item, pair, row0, n_rows, n_cols, ia, ib)) continue;
-        const int T = (n_cols + TC_BN - 1) / TC_BN;
-        const int ab = ai & 1;
-        tc::mbar_wait(&a_empty[ab], ((ai >> 1) & 1) ^ 1);
-        tc::mbar_expect_tx(&a_full[ab], 4 * TC_BOX_BYTES);
-        const int arow = ia * n_pad + row0;
+        int pair, col0, n_rows, n_cols, ia, ib;
+        if (!decode(item, pair, col0, n_rows, n_cols, ia, ib)) continue;
+        const int T = (n_rows + TC_BN - 1) / TC_BN;
+        const int bb = bi & 1;
+        tc::mbar_wait(&b_empty[bb], ((bi >> 1) & 1) ^ 1);
+        tc::mbar_expect_tx(&b_full[bb], 4 * TC_BOX_BYTES);
+        const int brow = ib * n_pad + col0;
         for (int slab = 0; slab < 2; ++slab)
           for (int kb = 0; kb < 2; ++kb)
-            tc::tma_load_2d(sA + ((ab * 2 + slab) * 2 + kb) * TC_BOX_BYTES, &maps.m1, &a_full[ab], kb * 64, arow + slab * 128);
-        ++ai;
-        const int brow = ib * n_pad;
-        for (int t = 0; t < T; ++t, ++bi) {
-          const int s = bi % TCF_NSB;
-          tc::mbar_wait(&b_empty[s], ((bi / TCF_NSB) & 1) ^ 1);
-          tc::mbar_expect_tx(&b_full[s], 2 * TC_BOX_BYTES);
+            tc::tma_load_2d(sB + ((bb * 2 + slab) * 2 + kb) * TC_BOX_BYTES, &maps.m2, &b_full[bb], kb * 64, brow + slab * 128);
+        ++bi;
+        const int arow = ia * n_pad;
+        for (int t = 0; t < T; ++t, ++ai) {
+          const int s = ai % TCF_NSA;
+          tc::mbar_wait(&a_empty[s], ((ai / TCF_NSA) & 1) ^ 1);
+          tc::mbar_expect_tx(&a_full[s], 2 * TC_BOX_BYTES);
           for (int kb = 0; kb < 2; ++kb)
-            tc::tma_load_2d(sB + (s * 2 + kb) * TC_BOX_BYTES, &maps.m2, &b_full[s], kb * 64, brow + t * TC_BN);
+            tc::tma_load_2d(sA + (s * 2 + kb) * TC_BOX_BYTES, &maps.m1, &a_full[s], kb * 64, arow + t * TC_BN);
         }
       }
     }
@@ -552,78 +595,73 @@ __global__ void __launch_bounds__(MT_THREADS, 1) mnn_tc_persist_kernel(const __g
   } else {
     const int slab = warp >> 2, wt = threadIdx.x & 127, cq = 2 * (lane & 3);
     const int my_turn = 1 + slab, next_turn = 2 - slab;   // named barriers: warpgroup 0 issues on 1, warpgroup 1 on 2
+    setmaxnreg_inc<232>();
     float acc0[64], acc1[64];
-    uint32_t ai = 0, bi = 0;
+    float cv[32];
+    int cr[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      cv[i] = -INFINITY;
+      cr[i] = 0;
+    }
+    uint32_t bi = 0, ai = 0;
     if (slab == 1) named_arrive(1, 256);   // warpgroup 0 goes first
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      int pair, row0, n_rows, n_cols, ia, ib;
-      if (!decode(item, pair, row0, n_rows, n_cols, ia, ib)) continue;
-      const int T = (n_cols + TC_BN - 1) / TC_BN;
-      const int ab = ai & 1;
-      const int srow0 = row0 + slab * 128;
-      bool rvalid[4];
-#pragma unroll
-      for (int h = 0; h < 4; ++h) rvalid[h] = srow0 + tc::frag_row(wt, h) < n_rows;
-      const bool rows_partial = srow0 + 128 > n_rows;
-      tc::mbar_wait(&a_full[ab], (ai >> 1) & 1);
-      const uint32_t a_slab = tc::smem_u32(sA + (ab * 2 + slab) * 2 * TC_BOX_BYTES);
-      float bv[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-      int bc[4] = {0, 0, 0, 0};
-      for (int t = 0; t < T; ++t, ++bi) {
-        const int s = bi % TCF_NSB;
-        tc::mbar_wait(&b_full[s], (bi / TCF_NSB) & 1);
+      int pair, col0, n_rows, n_cols, ia, ib;
+      if (!decode(item, pair, col0, n_rows, n_cols, ia, ib)) continue;
+      const int T = (n_rows + TC_BN - 1) / TC_BN;
+      const int bb = bi & 1;
+      const int scol0 = col0 + slab * TC_BN, n_valid = n_cols - scol0;   // n_valid <= 0: the whole slab lies past n2
+      unsigned long long* b12 = best12 + (int64_t)pair * n1_max;
+      tc::mbar_wait(&b_full[bb], (bi >> 1) & 1);
+      const uint32_t b_slab = tc::smem_u32(sB + (bb * 2 + slab) * 2 * TC_BOX_BYTES);
+      for (int t = 0; t < T; ++t, ++ai) {
+        const int s = ai % TCF_NSA;
+        tc::mbar_wait(&a_full[s], (ai / TCF_NSA) & 1);
         named_sync(my_turn, 256);
-        mnn_tile_mma_issue(acc0, acc1, a_slab, tc::smem_u32(sB + s * 2 * TC_BOX_BYTES), 0);
+        mnn_tile_mma_issue_halves(acc0, acc1, tc::smem_u32(sA + s * 2 * TC_BOX_BYTES), b_slab);
         named_arrive(next_turn, 256);
-        tc::wgmma_wait<0>();
+        int row[4];
+#pragma unroll
+        for (int h = 0; h < 4; ++h) row[h] = t * TC_BN + tc::frag_row(wt, h);
+        const bool rows_partial = (t + 1) * TC_BN > n_rows;
+        tc::wgmma_wait<1>();   // rows 0-63 of the tile are in acc0; rows 64-127 are still being computed
         tc::acc_fence(acc0);
+        mnn_half_epilogue<0>(acc0, row, scol0, n_valid, n_rows, rows_partial, lane, b12, cv, cr);
+        tc::wgmma_wait<0>();
         tc::acc_fence(acc1);
         __syncwarp();
         if (lane == 0) {
-          tc::mbar_arrive(&b_empty[s]);
-          if (t == T - 1) tc::mbar_arrive(&a_empty[ab]);   // the A slabs may be overwritten
+          tc::mbar_arrive(&a_empty[s]);
+          if (t == T - 1) tc::mbar_arrive(&b_empty[bb]);   // the B slabs may be overwritten
         }
-        const int col0 = t * TC_BN, n_valid = n_cols - col0;
-        if (n_valid < TC_BN) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-              if (8 * j + cq + e >= n_valid)
-#pragma unroll
-                for (int h = 0; h < 4; ++h) frag_ref(acc0, acc1, h, j, e) = -INFINITY;
-        }
-        if (rows_partial) {
-#pragma unroll
-          for (int h = 0; h < 4; ++h)
-            if (!rvalid[h])
-#pragma unroll
-              for (int j = 0; j < 16; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) frag_ref(acc0, acc1, h, j, e) = -INFINITY;
-        }
-        mnn_row_update(acc0, acc1, col0, lane, bv, bc);
-        float2* sc = sCol + (slab * 2 + (bi & 1)) * 4 * 128;
-        mnn_col_warp(acc0, acc1, wt, sc + (wt >> 5) * 128);
-        tc::wg_sync(3 + slab);   // the four warps' partials of this tile are in sc; parity bi & 1 is written again two tiles on
-        if (wt < n_valid) {
-          unsigned long long p = 0ull;
-#pragma unroll
-          for (int w = 0; w < 4; ++w) {
-            const float2 q = sc[w * 128 + wt];
-            if (q.x != -INFINITY) {
-              const unsigned long long c = pack_vi(q.x, (uint32_t)(srow0 + __float_as_int(q.y)));
-              p = c > p ? c : p;
-            }
-          }
-          if (p) atomicMax(best21 + (int64_t)pair * n2_max + col0 + wt, p);
-        }
+        mnn_half_epilogue<2>(acc1, row, scol0, n_valid, n_rows, rows_partial, lane, b12, cv, cr);
       }
-      ++ai;
-      if ((lane & 3) == 0) {
+      // the item's column partials: the 8 row lanes of a column, then the 4 warps; parity bi & 1 is written again two items on
+      unsigned long long* sc = sCol + (slab * 2 + bb) * 4 * 128;
 #pragma unroll
-        for (int h = 0; h < 4; ++h)
-          if (rvalid[h]) best12[(int64_t)pair * n1_max + srow0 + tc::frag_row(wt, h)] = pack_vi(bv[h], (uint32_t)bc[h]);
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          unsigned long long p = cv[2 * j + e] != -INFINITY ? pack_vi(cv[2 * j + e], (uint32_t)cr[2 * j + e]) : 0ull;
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            const unsigned long long q = __shfl_xor_sync(0xffffffffu, p, o);
+            p = q > p ? q : p;
+          }
+          if (lane < 4) sc[(wt >> 5) * 128 + 8 * j + cq + e] = p;
+          cv[2 * j + e] = -INFINITY;
+        }
+      ++bi;
+      tc::wg_sync(3 + slab);
+      if (wt < n_valid) {
+        unsigned long long p = sc[wt];
+#pragma unroll
+        for (int w = 1; w < 4; ++w) {
+          const unsigned long long q = sc[w * 128 + wt];
+          p = q > p ? q : p;
+        }
+        best21[(int64_t)pair * n2_max + scol0 + wt] = p;
       }
     }
     if (slab == 0) named_sync(1, 256);   // warpgroup 1's last hand-over
@@ -657,7 +695,7 @@ static int launch_mnn_tc_main(const TcMaps& maps, const int* n1, int n1_max, con
   } else {
     XF_DYN_SMEM(mnn_tc_persist_kernel, TCF_SMEM);
     const int n_items = batch * (n_pad / TC_ROWS);
-    mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, MT_THREADS, TCF_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
+    mnn_tc_persist_kernel<<<n_items < sms ? n_items : sms, TCF_THREADS, TCF_SMEM, st>>>(maps, n1, n1_max, n2, n2_max, n_pad, batch,
                                                                                       best12, best21, pairs);
   }
   XF_LAUNCH_CHECK();
