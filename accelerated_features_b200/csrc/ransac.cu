@@ -614,18 +614,313 @@ __device__ __forceinline__ int rs_f_sample(const float4* pts, const int (&idx)[7
   return rs_seven_point(F1, F2, Fc);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The five-point solver (Nistér 2004, "An efficient solution to the five-point relative pose problem"), fp64, no dynamic
+// allocation and a fixed iteration cap.  E = x N0 + y N1 + z N2 + N3 over the null space of the sample's five epipolar rows;
+// det(E) = 0 and 2 E E^T E - tr(E E^T) E = 0 are ten cubics in (x, y, z), stored over Nistér's order of the 20 monomials
+//   x^3 y^3 x^2y xy^2 x^2z x^2 y^2z y^2 xyz xy | xz^2 xz x yz^2 yz y z^3 z^2 z 1,
+// Gauss-Jordan eliminated on the first ten.  Rows (4, 5), (6, 7), (8, 9) then differ by a factor z in their leading monomials,
+// so row(2m+4) - z row(2m+5) is linear in (x, y, 1) with polynomial coefficients in z; the determinant of those three rows is a
+// degree-10 polynomial whose real roots (Sturm sequence + bisection, then safeguarded Newton) give z, and the null vector of
+// the 3 x 3 system gives (x, y).  __host__ so that the host build can run the same arithmetic.
+// ---------------------------------------------------------------------------------------------------------------------
+
+// q += s * a * b: two linear forms over (x, y, z, 1) into a quadratic over (x^2, y^2, z^2, xy, xz, yz, x, y, z, 1)
+__host__ __device__ __forceinline__ void rs_mul11(const double (&a)[4], const double (&b)[4], double s, double (&q)[10]) {
+  const int Q[4][4] = {{0, 3, 4, 6}, {3, 1, 5, 7}, {4, 5, 2, 8}, {6, 7, 8, 9}};
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) q[Q[i][j]] += s * a[i] * b[j];
+}
+
+// c += s * q * a: a quadratic times a linear form into a cubic over the 20 monomials above
+__host__ __device__ __forceinline__ void rs_mul21(const double (&q)[10], const double (&a)[4], double s, double (&c)[20]) {
+  const int C[10][4] = {{0, 2, 4, 5},    {3, 1, 6, 7},     {10, 13, 16, 17}, {2, 3, 8, 9},     {4, 8, 10, 11},
+                        {8, 6, 13, 14},  {5, 9, 11, 12},   {9, 7, 14, 15},   {11, 14, 17, 18}, {12, 15, 18, 19}};
+#pragma unroll
+  for (int i = 0; i < 10; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) c[C[i][j]] += s * q[i] * a[j];
+}
+
+// c = a * b (ascending powers of z)
+template <int NA, int NB>
+__host__ __device__ __forceinline__ void rs_pmul(const double (&a)[NA], const double (&b)[NB], double (&c)[NA + NB - 1]) {
+  for (int k = 0; k < NA + NB - 1; ++k) c[k] = 0.0;
+  for (int i = 0; i < NA; ++i)
+    for (int j = 0; j < NB; ++j) c[i + j] += a[i] * b[j];
+}
+
+__host__ __device__ __forceinline__ double rs_horner(const double* c, int deg, double x) {
+  double v = c[deg];
+  for (int k = deg - 1; k >= 0; --k) v = v * x + c[k];
+  return v;
+}
+
+constexpr int RS_ROOT_BISECT = 80;     // Sturm bisection steps per root (isolates roots 2e7 / 2^80 apart)
+constexpr int RS_ROOT_POLISH = 100;    // bisection + safeguarded Newton steps per isolated root
+constexpr double RS_ROOT_BOUND = 1e7;  // |z| beyond this (E nearly without an N3 component) is not searched
+constexpr int RS_ROOT_DET_NEWTON = 3;  // Newton steps per root on the unexpanded determinant
+
+__host__ __device__ __forceinline__ double rs_det3(const double* r0, const double* r1, const double* r2) {
+  return r0[0] * (r1[1] * r2[2] - r1[2] * r2[1]) - r0[1] * (r1[0] * r2[2] - r1[2] * r2[0]) + r0[2] * (r1[0] * r2[1] - r1[1] * r2[0]);
+}
+
+// Sign changes of the Sturm sequence S[0..ns-1] (degrees dg) at x.
+__host__ __device__ __forceinline__ int rs_sturm_changes(const double (&S)[11][11], const int (&dg)[11], int ns, double x) {
+  int changes = 0, last = 0;
+  for (int i = 0; i < ns; ++i) {
+    const double v = rs_horner(S[i], dg[i], x);
+    const int s = v > 0.0 ? 1 : (v < 0.0 ? -1 : 0);
+    if (s != 0) {
+      if (last != 0 && s != last) ++changes;
+      last = s;
+    }
+  }
+  return changes;
+}
+
+// The distinct real roots in (-RS_ROOT_BOUND, RS_ROOT_BOUND) of the polynomial c (ascending, degree <= 10), ascending.
+__host__ __device__ int rs_real_roots(const double (&c)[11], double (&roots)[10]) {
+  double amax = 0.0;
+  for (int k = 0; k <= 10; ++k) amax = fmax(amax, fabs(c[k]));
+  if (!(amax > 1e-300) || !isfinite(amax)) return 0;
+  int d = 10;
+  while (d > 0 && fabs(c[d]) <= 1e-14 * amax) --d;   // leading terms at rounding level: those roots are at infinity
+  if (d == 0) return 0;
+  double S[11][11];
+  int dg[11];
+  for (int k = 0; k <= d; ++k) S[0][k] = c[k] / amax;
+  dg[0] = d;
+  double dmax = 0.0;
+  for (int k = 1; k <= d; ++k) dmax = fmax(dmax, fabs(k * S[0][k]));
+  for (int k = 1; k <= d; ++k) S[1][k - 1] = k * S[0][k] / dmax;
+  dg[1] = d - 1;
+  int ns = 2;
+  while (ns < 11 && dg[ns - 1] > 0) {                  // S[i+1] = -(S[i-1] mod S[i]), each scaled to max |coefficient| 1
+    double r[11];
+    const int da = dg[ns - 2], db = dg[ns - 1];
+    for (int k = 0; k <= da; ++k) r[k] = S[ns - 2][k];
+    for (int k = da; k >= db; --k) {
+      const double q = r[k] / S[ns - 1][db];
+      for (int j = 0; j <= db; ++j) r[k - db + j] -= q * S[ns - 1][j];
+    }
+    int dr = db - 1;
+    double rmax = 0.0;
+    for (int k = 0; k <= dr; ++k) rmax = fmax(rmax, fabs(r[k]));
+    if (!(rmax > 1e-12)) break;                        // S[ns-1] divides S[ns-2]: a repeated root; the count stays exact
+    while (dr > 0 && fabs(r[dr]) <= 1e-14 * rmax) --dr;
+    for (int k = 0; k <= dr; ++k) S[ns][k] = -r[k] / rmax;
+    dg[ns] = dr;
+    ++ns;
+  }
+  double bound = 0.0;                                  // Cauchy bound of the roots
+  for (int k = 0; k < d; ++k) bound = fmax(bound, fabs(S[0][k] / S[0][d]));
+  bound = fmin(1.0 + bound, RS_ROOT_BOUND);
+  const int v_lo = rs_sturm_changes(S, dg, ns, -bound);
+  const int total = min(max(v_lo - rs_sturm_changes(S, dg, ns, bound), 0), 10);
+  double lo = -bound;
+  int c_lo = 0;                                        // roots <= lo
+  int nr = 0;
+  for (int k = 0; k < total; ++k) {
+    double hi = bound;
+    int c_hi = total;
+    for (int it = 0; it < RS_ROOT_BISECT && (c_hi - c_lo > 1 || c_lo != k); ++it) {
+      const double mid = 0.5 * (lo + hi);
+      const int cm = v_lo - rs_sturm_changes(S, dg, ns, mid);
+      if (cm > k) { hi = mid; c_hi = cm; }
+      else { lo = mid; c_lo = cm; }
+    }
+    // the k-th root is alone in (lo, hi]: bisection on the sign of S[0] down to a narrow bracket (an isolating interval can
+    // be as wide as the search range), then Newton steps kept inside the bracket
+    double a = lo, b = hi, fa = rs_horner(S[0], d, a);
+    double x = 0.5 * (a + b);
+    for (int it = 0; it < RS_ROOT_POLISH; ++it) {
+      const double f = rs_horner(S[0], d, x);
+      if (f == 0.0) break;
+      if ((f > 0.0) == (fa > 0.0)) { a = x; fa = f; } else { b = x; }
+      double xn = 0.5 * (a + b);
+      if (b - a < 1e-3 * fmax(1.0, fabs(x))) {
+        double df = 0.0;
+        for (int j = d; j >= 1; --j) df = df * x + j * S[0][j];
+        const double xt = x - f / df;
+        if (xt > a && xt < b) xn = xt;
+      }
+      if (fabs(xn - x) <= 1e-15 * fmax(1.0, fabs(x))) { x = xn; break; }
+      x = xn;
+    }
+    roots[nr++] = x;
+    lo = hi;
+    c_lo = c_hi;
+  }
+  return nr;
+}
+
+// The five-point step on a null-space basis N (four 3 x 3 matrices, row-major): 0-10 candidates, unit Frobenius norm.
+__host__ __device__ int rs_five_point(const double (&N)[4][9], float (&Ec)[10][9]) {
+  double L[9][4];                                      // entry k of E as a linear form over (x, y, z, 1)
+  for (int k = 0; k < 9; ++k)
+    for (int j = 0; j < 4; ++j) L[k][j] = N[j][k];
+  double A[10][20];
+  for (int r = 0; r < 10; ++r)
+    for (int k = 0; k < 20; ++k) A[r][k] = 0.0;
+  {                                                    // det(E), along the first row
+    const int cof[3][4] = {{4, 8, 5, 7}, {5, 6, 3, 8}, {3, 7, 4, 6}};
+    for (int c = 0; c < 3; ++c) {
+      double q[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+      rs_mul11(L[cof[c][0]], L[cof[c][1]], 1.0, q);
+      rs_mul11(L[cof[c][2]], L[cof[c][3]], -1.0, q);
+      rs_mul21(q, L[c], 1.0, A[0]);
+    }
+  }
+  double P[3][3][10];                                  // E E^T
+  double tr[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      for (int k = 0; k < 10; ++k) P[i][j][k] = 0.0;
+      for (int k = 0; k < 3; ++k) rs_mul11(L[3 * i + k], L[3 * j + k], 1.0, P[i][j]);
+    }
+  for (int i = 0; i < 3; ++i)
+    for (int k = 0; k < 10; ++k) tr[k] += P[i][i][k];
+  for (int i = 0; i < 3; ++i)                          // 2 E E^T E - tr(E E^T) E
+    for (int j = 0; j < 3; ++j) {
+      for (int k = 0; k < 3; ++k) rs_mul21(P[i][k], L[3 * k + j], 2.0, A[1 + 3 * i + j]);
+      rs_mul21(tr, L[3 * i + j], -1.0, A[1 + 3 * i + j]);
+    }
+  double amax = 0.0;
+  for (int r = 0; r < 10; ++r)
+    for (int k = 0; k < 20; ++k) amax = fmax(amax, fabs(A[r][k]));
+  if (!(amax > 1e-300) || !isfinite(amax)) return 0;
+  for (int c = 0; c < 10; ++c) {                       // Gauss-Jordan with partial pivoting on the ten leading monomials
+    int piv = c;
+    for (int r = c + 1; r < 10; ++r)
+      if (fabs(A[r][c]) > fabs(A[piv][c])) piv = r;
+    if (!(fabs(A[piv][c]) > 1e-11 * amax)) return 0;  // rank-deficient: repeated or degenerate points
+    if (piv != c)
+      for (int k = c; k < 20; ++k) { const double t = A[c][k]; A[c][k] = A[piv][k]; A[piv][k] = t; }
+    const double inv = 1.0 / A[c][c];
+    for (int k = c; k < 20; ++k) A[c][k] *= inv;
+    for (int r = 0; r < 10; ++r) {
+      if (r == c) continue;
+      const double f = A[r][c];
+      for (int k = c; k < 20; ++k) A[r][k] -= f * A[c][k];
+    }
+  }
+  double bx[3][4], by[3][4], b1[3][5];                 // rows (2m+4) - z (2m+5): coefficients of x, y and 1 in z
+  for (int m = 0; m < 3; ++m) {
+    const double* e = A[4 + 2 * m];
+    const double* f = A[5 + 2 * m];
+    bx[m][0] = e[12]; bx[m][1] = e[11] - f[12]; bx[m][2] = e[10] - f[11]; bx[m][3] = -f[10];
+    by[m][0] = e[15]; by[m][1] = e[14] - f[15]; by[m][2] = e[13] - f[14]; by[m][3] = -f[13];
+    b1[m][0] = e[19]; b1[m][1] = e[18] - f[19]; b1[m][2] = e[17] - f[18]; b1[m][3] = e[16] - f[17]; b1[m][4] = -f[16];
+  }
+  double p[11];
+  {
+    double u[8], v[8], w[7], t[11];
+    rs_pmul(by[1], b1[2], u); rs_pmul(b1[1], by[2], v);
+    for (int k = 0; k < 8; ++k) u[k] -= v[k];
+    rs_pmul(bx[0], u, p);
+    rs_pmul(bx[1], b1[2], u); rs_pmul(b1[1], bx[2], v);
+    for (int k = 0; k < 8; ++k) u[k] -= v[k];
+    rs_pmul(by[0], u, t);
+    for (int k = 0; k < 11; ++k) p[k] -= t[k];
+    double w2[7];
+    rs_pmul(bx[1], by[2], w); rs_pmul(by[1], bx[2], w2);
+    for (int k = 0; k < 7; ++k) w[k] -= w2[k];
+    rs_pmul(b1[0], w, t);
+    for (int k = 0; k < 11; ++k) p[k] += t[k];
+  }
+  double z[10];
+  const int nz = rs_real_roots(p, z);
+  int nc = 0;
+  for (int j = 0; j < nz; ++j) {
+    double B[3][3];
+    // Newton on det B(z) evaluated from B's entries: the expanded degree-10 coefficients cancel badly when roots cluster
+    for (int it = 0; it < RS_ROOT_DET_NEWTON; ++it) {
+      double D[3][3];
+      for (int m = 0; m < 3; ++m) {
+        B[m][0] = rs_horner(bx[m], 3, z[j]); B[m][1] = rs_horner(by[m], 3, z[j]); B[m][2] = rs_horner(b1[m], 4, z[j]);
+        D[m][0] = (3.0 * bx[m][3] * z[j] + 2.0 * bx[m][2]) * z[j] + bx[m][1];
+        D[m][1] = (3.0 * by[m][3] * z[j] + 2.0 * by[m][2]) * z[j] + by[m][1];
+        D[m][2] = ((4.0 * b1[m][4] * z[j] + 3.0 * b1[m][3]) * z[j] + 2.0 * b1[m][2]) * z[j] + b1[m][1];
+      }
+      const double f = rs_det3(B[0], B[1], B[2]);
+      const double df = rs_det3(D[0], B[1], B[2]) + rs_det3(B[0], D[1], B[2]) + rs_det3(B[0], B[1], D[2]);
+      const double step = f / df;
+      if (!(fabs(step) < 1e-3 * fmax(1.0, fabs(z[j])))) break;   // not converging here: keep the polynomial's root
+      z[j] -= step;
+    }
+    for (int m = 0; m < 3; ++m) {
+      B[m][0] = rs_horner(bx[m], 3, z[j]); B[m][1] = rs_horner(by[m], 3, z[j]); B[m][2] = rs_horner(b1[m], 4, z[j]);
+    }
+    double v[3] = {0.0, 0.0, 0.0}, vn = -1.0;          // (x, y, 1): the largest cross product of two rows
+    for (int a = 0; a < 3; ++a) {
+      const double* r0 = B[a];
+      const double* r1 = B[(a + 1) % 3];
+      const double cr[3] = {r0[1] * r1[2] - r0[2] * r1[1], r0[2] * r1[0] - r0[0] * r1[2], r0[0] * r1[1] - r0[1] * r1[0]};
+      const double n2 = cr[0] * cr[0] + cr[1] * cr[1] + cr[2] * cr[2];
+      if (n2 > vn) { vn = n2; v[0] = cr[0]; v[1] = cr[1]; v[2] = cr[2]; }
+    }
+    if (!(fabs(v[2]) > 1e-12 * sqrt(vn))) continue;
+    const double x = v[0] / v[2], y = v[1] / v[2];
+    double E[9], nrm = 0.0;
+    for (int k = 0; k < 9; ++k) { E[k] = x * N[0][k] + y * N[1][k] + z[j] * N[2][k] + N[3][k]; nrm += E[k] * E[k]; }
+    if (!(nrm > 1e-300) || !isfinite(nrm)) continue;
+    const double inv = 1.0 / sqrt(nrm);
+    for (int k = 0; k < 9; ++k) Ec[nc][k] = (float)(E[k] * inv);
+    ++nc;
+  }
+  return nc;
+}
+
+// One 5-point sample, the body of a relative-pose hypothesis lane: the 9 x 9 normal matrix of the five epipolar rows of
+// pts[idx[0..4]] (calibrated (x, y, u, v)), its four smallest eigenvectors (cyclic Jacobi) as the null space, and the 0-10
+// candidates of rs_five_point.  Also run on its own by xfeat_debug_five_point.
+__device__ __forceinline__ int rs_e5_sample(const float4* pts, const int (&idx)[5], float (&Ec)[10][9]) {
+  double M[9][9];
+  rs_epi_normal<5>(pts, idx, M);
+  double V[9][9];
+  rs_jacobi<9>(M, V);
+  bool used[9] = {false, false, false, false, false, false, false, false, false};
+  double N[4][9];
+  for (int j = 0; j < 4; ++j) {                        // the four smallest eigenvalues, ascending
+    int lo = -1;
+    for (int i = 0; i < 9; ++i)
+      if (!used[i] && (lo < 0 || M[i][i] < M[lo][lo])) lo = i;
+    used[lo] = true;
+    for (int k = 0; k < 9; ++k) N[j][k] = V[k][lo];
+  }
+  double l5 = 3.0e300, lmax = 0.0;                     // five independent rows, or the null space is not 4-D
+  for (int i = 0; i < 9; ++i) {
+    lmax = fmax(lmax, M[i][i]);
+    if (!used[i]) l5 = fmin(l5, M[i][i]);
+  }
+  if (!(l5 > 1e-13 * lmax)) return 0;                   // repeated points
+  return rs_five_point(N, Ec);
+}
+
+// Per-pair intrinsics of the calibrated model: K0, K1 (batch, 4) as (fx, fy, cx, cy); null for the other models.
+struct RsCams {
+  const float* K0;
+  const float* K1;
+};
+
 // What the epipolar kernels need to know about a model:
 //   kSample, kCands     minimal sample size, candidates per sample
+//   kMinPts             fewest correspondences a pair needs for a model (below it: no model)
 //   kLoMinBlocks        minimum blocks per SM in the local-optimisation kernel's launch bound (0: none)
-//   Norm, prepare()     caches the pair's correspondences in sPts (visible to the block on return) and returns the squared
+//   Norm, camera()      what the model keeps per pair; camera() loads the pair's intrinsics into it (a no-op without)
+//   prepare()           caches the pair's correspondences in sPts (visible to the block on return) and returns the squared
 //                       threshold in the cached frame
 //   solve()             one lane's sample -> candidates (unit-scale float models in the cached frame)
 //   project()           the constraint every local-optimisation refit is projected onto
 //   to_output()         a model of the cached frame -> the record's output model
 //   inlier()            the final classification on the caller's coordinates
 struct RsEssential {
-  static constexpr int kSample = 8, kCands = 1, kLoMinBlocks = 0;
+  static constexpr int kSample = 8, kCands = 1, kMinPts = 8, kLoMinBlocks = 0;
   struct Norm {};
+  static __device__ __forceinline__ void camera(const RsCams&, int, Norm&) {}
   static __device__ __forceinline__ float prepare(const float* __restrict__ q0, const float* __restrict__ q1, int n, float thr,
                                                   float4* sPts, Norm&) {
     for (int i = threadIdx.x; i < n; i += RS_THREADS) sPts[i] = make_float4(q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1]);
@@ -644,7 +939,7 @@ struct RsEssential {
   static __device__ __forceinline__ void to_output(const Norm&, const float* sE, float* out) {
     for (int k = 0; k < 9; ++k) out[k] = sE[k];
   }
-  static __device__ __forceinline__ bool inlier(const float (&E)[9], float x, float y, float u, float v, float thr) {
+  static __device__ __forceinline__ bool inlier(const Norm&, const float (&E)[9], float x, float y, float u, float v, float thr) {
     return rs_sampson2(E, x, y, u, v) < thr * thr;
   }
 };
@@ -652,8 +947,9 @@ struct RsEssential {
 struct RsFundamental {
   // One block per SM in the local optimisation's launch bound: under the default, ptxas caps that kernel at 128 registers and
   // spills.
-  static constexpr int kSample = 7, kCands = 3, kLoMinBlocks = 1;
+  static constexpr int kSample = 7, kCands = 3, kMinPts = 8, kLoMinBlocks = 1;
   using Norm = RsPairNorm;
+  static __device__ __forceinline__ void camera(const RsCams&, int, Norm&) {}
   static __device__ __forceinline__ float prepare(const float* __restrict__ q0, const float* __restrict__ q1, int n, float thr,
                                                   float4* sPts, Norm& nz) {
     nz = rs_pair_normalise(q0, q1, n, sPts);
@@ -679,8 +975,48 @@ struct RsFundamental {
     const double inv = nrm > 1e-300 ? 1.0 / sqrt(nrm) : 0.0;
     for (int k = 0; k < 9; ++k) out[k] = (float)(F[k] * inv);
   }
-  static __device__ __forceinline__ bool inlier(const float (&F)[9], float x, float y, float u, float v, float thr) {
+  static __device__ __forceinline__ bool inlier(const Norm&, const float (&F)[9], float x, float y, float u, float v, float thr) {
     return rs_sampson2_px(F, x, y, u, v) < (double)thr * (double)thr;
+  }
+};
+
+// Calibrated relative pose (what poselib.estimate_relative_pose runs in the 1500-pair benchmarks, modules/eval/megadepth1500.py:
+// 98-113, minus its non-linear refinement).  Inputs are PIXELS with per-pair intrinsics; prepare() caches K^-1-normalised
+// coordinates, the minimal solver is the five-point algorithm (0-10 candidates, planar scenes included), and thr (pixels)
+// becomes thr / f with f = (fx0 + fy0 + fx1 + fy1) / 4, the rule of evalharness.estimate_pose_opencv.  Inliers: Sampson
+// distance in normalised coordinates, as RsEssential.
+struct RsEssential5 {
+  static constexpr int kSample = 5, kCands = 10, kMinPts = 5, kLoMinBlocks = 0;
+  struct Norm { float fx0, fy0, cx0, cy0, fx1, fy1, cx1, cy1; };
+  static __device__ __forceinline__ void camera(const RsCams& c, int pair, Norm& nz) {
+    const float* a = c.K0 + 4 * pair;
+    const float* b = c.K1 + 4 * pair;
+    nz = Norm{a[0], a[1], a[2], a[3], b[0], b[1], b[2], b[3]};
+  }
+  static __device__ __forceinline__ float threshold(const Norm& nz, float thr) {
+    return thr / (0.25f * (nz.fx0 + nz.fy0 + nz.fx1 + nz.fy1));
+  }
+  static __device__ __forceinline__ float4 normalise(const Norm& nz, float x, float y, float u, float v) {
+    return make_float4((x - nz.cx0) / nz.fx0, (y - nz.cy0) / nz.fy0, (u - nz.cx1) / nz.fx1, (v - nz.cy1) / nz.fy1);
+  }
+  static __device__ __forceinline__ float prepare(const float* __restrict__ q0, const float* __restrict__ q1, int n, float thr,
+                                                  float4* sPts, Norm& nz) {
+    for (int i = threadIdx.x; i < n; i += RS_THREADS) sPts[i] = normalise(nz, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1]);
+    __syncthreads();
+    const float t = threshold(nz, thr);
+    return t * t;
+  }
+  static __device__ __forceinline__ int solve(const float4* pts, const int (&idx)[kSample], float (&Ec)[kCands][9]) {
+    return rs_e5_sample(pts, idx, Ec);
+  }
+  static __device__ __forceinline__ void project(double (&E)[9]) { rs_project_essential(E); }
+  static __device__ __forceinline__ void to_output(const Norm&, const float* sE, float* out) {
+    for (int k = 0; k < 9; ++k) out[k] = sE[k];
+  }
+  static __device__ __forceinline__ bool inlier(const Norm& nz, const float (&E)[9], float x, float y, float u, float v, float thr) {
+    const float4 c = normalise(nz, x, y, u, v);
+    const float t = threshold(nz, thr);
+    return rs_sampson2(E, c.x, c.y, c.z, c.w) < t * t;
   }
 };
 
@@ -762,8 +1098,8 @@ __device__ __forceinline__ float rs_local_opt(const float4* __restrict__ sPts, i
 template <class Model>
 __global__ void __launch_bounds__(RS_THREADS) ransac_hyp_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
                                                                 const int* __restrict__ np, const int* __restrict__ pair_ids,
-                                                                int n_max, float thr, int rounds_per_warp, uint32_t seed,
-                                                                RsRecord* __restrict__ best) {
+                                                                RsCams cams, int n_max, float thr, int rounds_per_warp,
+                                                                uint32_t seed, RsRecord* __restrict__ best) {
   extern __shared__ float4 sPts[];                 // (x, y, u, v) in the model's frame
   const int pair = blockIdx.y;
   const int n = min(np ? np[pair] : n_max, min(n_max, RS_MAX_PTS));
@@ -772,8 +1108,9 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_hyp_kernel(const float* __r
 #pragma unroll
   for (int k = 0; k < 9; ++k) mine.m[k] = 0.f;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (n >= 8) {
+  if (n >= Model::kMinPts) {
     typename Model::Norm nz;
+    Model::camera(cams, pair, nz);
     const float t2 = Model::prepare(p0 + (int64_t)pair * n_max * 2, p1 + (int64_t)pair * n_max * 2, n, thr, sPts, nz);
     const uint32_t pid = pair_ids ? (uint32_t)pair_ids[pair] : (uint32_t)pair;
     for (int rd = 0; rd < rounds_per_warp; ++rd) {
@@ -815,16 +1152,18 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_hyp_kernel(const float* __r
 template <class Model>
 __global__ void __launch_bounds__(RS_THREADS, Model::kLoMinBlocks) ransac_lo_kernel(const float* __restrict__ p0,
                                                                                     const float* __restrict__ p1,
-                                                                                    const int* __restrict__ np, int n_max,
-                                                                                    float thr, RsRecord* __restrict__ best) {
+                                                                                    const int* __restrict__ np, RsCams cams,
+                                                                                    int n_max, float thr,
+                                                                                    RsRecord* __restrict__ best) {
   extern __shared__ float4 sPts[];
   __shared__ float sE[9];
   const int pair = blockIdx.y;
   const int n = min(np ? np[pair] : n_max, min(n_max, RS_MAX_PTS));
-  if (n < 8) return;
+  if (n < Model::kMinPts) return;
   RsRecord* rec = best + (int64_t)pair * gridDim.x + blockIdx.x;
   if (!(rec->cost < RS_NO_COST)) return;             // this block found no hypothesis (block-uniform)
   typename Model::Norm nz;
+  Model::camera(cams, pair, nz);
   const float t2 = Model::prepare(p0 + (int64_t)pair * n_max * 2, p1 + (int64_t)pair * n_max * 2, n, thr, sPts, nz);
   if (threadIdx.x < 9) sE[threadIdx.x] = rec->m[threadIdx.x];
   const float cost = rs_local_opt<Model>(sPts, n, t2, sE);
@@ -837,20 +1176,22 @@ __global__ void __launch_bounds__(RS_THREADS, Model::kLoMinBlocks) ransac_lo_ker
 // stage 3: one block per pair: the best optimised candidate classifies the correspondences (Model::inlier) -> model, mask, count.
 template <class Model>
 __global__ void __launch_bounds__(RS_THREADS) ransac_final_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
-                                                                  const int* __restrict__ np, int n_max, float thr,
-                                                                  const RsRecord* __restrict__ best, int blocks_per_pair,
-                                                                  float* __restrict__ M_out, unsigned char* __restrict__ mask,
-                                                                  int* __restrict__ n_inl) {
+                                                                  const int* __restrict__ np, RsCams cams, int n_max,
+                                                                  float thr, const RsRecord* __restrict__ best,
+                                                                  int blocks_per_pair, float* __restrict__ M_out,
+                                                                  unsigned char* __restrict__ mask, int* __restrict__ n_inl) {
   __shared__ float sM[9];
   const int pair = blockIdx.x;
   const int n_all = np ? np[pair] : n_max;
   const int n = min(n_all, min(n_max, RS_MAX_PTS));
   unsigned char* mk = mask + (int64_t)pair * n_max;
   for (int i = threadIdx.x; i < n_max; i += RS_THREADS) mk[i] = 0;
-  if (n < 8) {
+  if (n < Model::kMinPts) {
     if (threadIdx.x == 0) rs_write_none(n_all, 0.f, M_out + pair * 9, n_inl + pair);
     return;
   }
+  typename Model::Norm nz;
+  Model::camera(cams, pair, nz);
   const float* q0 = p0 + (int64_t)pair * n_max * 2;
   const float* q1 = p1 + (int64_t)pair * n_max * 2;
   if (threadIdx.x == 0) {
@@ -863,7 +1204,7 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_final_kernel(const float* _
   for (int k = 0; k < 9; ++k) m[k] = sM[k];
   int cnt = 0;
   for (int i = threadIdx.x; i < n; i += RS_THREADS) {
-    const bool in = Model::inlier(m, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1], thr);
+    const bool in = Model::inlier(nz, m, q0[2 * i], q0[2 * i + 1], q1[2 * i], q1[2 * i + 1], thr);
     mk[i] = in ? 1 : 0;
     cnt += in ? 1 : 0;
   }
@@ -872,6 +1213,125 @@ __global__ void __launch_bounds__(RS_THREADS) ransac_final_kernel(const float* _
     n_inl[pair] = cnt;
     for (int k = 0; k < 9; ++k) M_out[pair * 9 + k] = m[k];
   }
+}
+
+// stage 4 of the relative pose: one block per pair.  The four (R, t) decompositions of the pair's E in geometry.recover_pose's
+// order -- (R1, t), (R1, -t), (R2, t), (R2, -t) with E = U diag(1, 1, 0) V^T, det U = det V = +1, R1 = U W V^T,
+// R2 = U W^T V^T, t = U[:, 2] -- and for each, the RANSAC inliers triangulated by the same 2 x 2 least-squares depth solve
+// (z0 R x0 - z1 x1 = -t, normal equations + 1e-12 I), in fp64; the candidate with the most points in front of both cameras wins,
+// the first in that order on a tie.  A pair without a model (no inliers) gets R = I, t = 0, n_front = 0.
+__global__ void __launch_bounds__(RS_THREADS) ransac_pose_kernel(const float* __restrict__ p0, const float* __restrict__ p1,
+                                                                 const int* __restrict__ np, RsCams cams, int n_max,
+                                                                 const float* __restrict__ E_in,
+                                                                 const unsigned char* __restrict__ mask,
+                                                                 const int* __restrict__ n_inl, float* __restrict__ R_out,
+                                                                 float* __restrict__ t_out, int* __restrict__ n_front) {
+  __shared__ double sR[2][9], sT[3];
+  __shared__ int sOk;
+  const int pair = blockIdx.x;
+  const int n = min(np ? np[pair] : n_max, min(n_max, RS_MAX_PTS));
+  if (threadIdx.x == 0) {
+    double E[9], M[3][3], V[3][3];
+    for (int k = 0; k < 9; ++k) E[k] = E_in[pair * 9 + k];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) M[i][j] = E[i] * E[j] + E[3 + i] * E[3 + j] + E[6 + i] * E[6 + j];
+    rs_jacobi<3>(M, V);
+    int o[3] = {0, 1, 2};                              // singular values descending
+    for (int a = 0; a < 3; ++a)
+      for (int b = a + 1; b < 3; ++b)
+        if (M[o[b]][o[b]] > M[o[a]][o[a]]) { const int t = o[a]; o[a] = o[b]; o[b] = t; }
+    double v[3][3], u[3][3];                           // v[c], u[c]: column c of V, U
+    for (int c = 0; c < 3; ++c)
+      for (int r = 0; r < 3; ++r) v[c][r] = V[r][o[c]];
+    const double dv = v[0][0] * (v[1][1] * v[2][2] - v[1][2] * v[2][1]) - v[0][1] * (v[1][0] * v[2][2] - v[1][2] * v[2][0]) +
+                      v[0][2] * (v[1][0] * v[2][1] - v[1][1] * v[2][0]);
+    if (dv < 0.0)
+      for (int r = 0; r < 3; ++r) v[2][r] = -v[2][r];
+    double s[2];
+    for (int c = 0; c < 2; ++c) {                      // u_c = E v_c, u_1 orthogonalised against u_0
+      for (int r = 0; r < 3; ++r) u[c][r] = E[3 * r] * v[c][0] + E[3 * r + 1] * v[c][1] + E[3 * r + 2] * v[c][2];
+      if (c == 1) {
+        const double d = u[0][0] * u[1][0] + u[0][1] * u[1][1] + u[0][2] * u[1][2];
+        for (int r = 0; r < 3; ++r) u[1][r] -= d * u[0][r];
+      }
+      s[c] = sqrt(u[c][0] * u[c][0] + u[c][1] * u[c][1] + u[c][2] * u[c][2]);
+      if (s[c] > 1e-300)
+        for (int r = 0; r < 3; ++r) u[c][r] /= s[c];
+    }
+    u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];   // det U = +1
+    u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
+    u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+    sOk = n_inl[pair] > 0 && s[0] > 1e-300 && s[1] > 1e-300;
+    // R = U W V^T = u0 (W^T row 0) ... : W = [[0,-1,0],[1,0,0],[0,0,1]] maps columns: U W = [u1, -u0, u2], U W^T = [-u1, u0, u2]
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) {
+        sR[0][3 * i + j] = u[1][i] * v[0][j] - u[0][i] * v[1][j] + u[2][i] * v[2][j];
+        sR[1][3 * i + j] = -u[1][i] * v[0][j] + u[0][i] * v[1][j] + u[2][i] * v[2][j];
+      }
+    for (int r = 0; r < 3; ++r) sT[r] = u[2][r];
+  }
+  __syncthreads();
+  if (!sOk) {
+    if (threadIdx.x < 9) R_out[pair * 9 + threadIdx.x] = (threadIdx.x % 4 == 0) ? 1.f : 0.f;
+    if (threadIdx.x < 3) t_out[pair * 3 + threadIdx.x] = 0.f;
+    if (threadIdx.x == 0) n_front[pair] = 0;
+    return;
+  }
+  RsEssential5::Norm nz;
+  RsEssential5::camera(cams, pair, nz);
+  const float* q0 = p0 + (int64_t)pair * n_max * 2;
+  const float* q1 = p1 + (int64_t)pair * n_max * 2;
+  const unsigned char* mk = mask + (int64_t)pair * n_max;
+  int cnt[4] = {0, 0, 0, 0};
+  for (int i = threadIdx.x; i < n; i += RS_THREADS) {
+    if (!mk[i]) continue;
+    const double h0[3] = {((double)q0[2 * i] - nz.cx0) / nz.fx0, ((double)q0[2 * i + 1] - nz.cy0) / nz.fy0, 1.0};
+    const double h1[3] = {((double)q1[2 * i] - nz.cx1) / nz.fx1, ((double)q1[2 * i + 1] - nz.cy1) / nz.fy1, 1.0};
+    const double h11 = h1[0] * h1[0] + h1[1] * h1[1] + 1.0 + 1e-12;
+    const double h1t = h1[0] * sT[0] + h1[1] * sT[1] + h1[2] * sT[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const double* R = sR[r];
+      double a[3];
+      for (int k = 0; k < 3; ++k) a[k] = R[3 * k] * h0[0] + R[3 * k + 1] * h0[1] + R[3 * k + 2];
+      const double aa = a[0] * a[0] + a[1] * a[1] + a[2] * a[2] + 1e-12, ah = -(a[0] * h1[0] + a[1] * h1[1] + a[2]);
+      const double at = a[0] * sT[0] + a[1] * sT[1] + a[2] * sT[2];
+      const double det = aa * h11 - ah * ah;
+#pragma unroll
+      for (int sg = 0; sg < 2; ++sg) {               // A = [a, -h1], b = -(+-t): A^T b = (-+ a.t, +- h1.t)
+        const double b0 = sg == 0 ? -at : at, b1 = sg == 0 ? h1t : -h1t;
+        const double z0 = (h11 * b0 - ah * b1) / det, z1 = (aa * b1 - ah * b0) / det;
+        cnt[2 * r + sg] += (z0 > 0.0 && z1 > 0.0) ? 1 : 0;
+      }
+    }
+  }
+  int tot[4];
+  for (int c = 0; c < 4; ++c) {
+    tot[c] = rs_block_count(cnt[c]);
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    int best = 0;
+    for (int c = 1; c < 4; ++c)
+      if (tot[c] > tot[best]) best = c;
+    const double sg = (best & 1) ? -1.0 : 1.0;
+    for (int k = 0; k < 9; ++k) R_out[pair * 9 + k] = (float)sR[best >> 1][k];
+    for (int k = 0; k < 3; ++k) t_out[pair * 3 + k] = (float)(sg * sT[k]);
+    n_front[pair] = tot[best];
+  }
+}
+
+// Test hook: one thread per 5-point sample (5 calibrated (x, y, u, v) rows), candidates zero-padded to 10.
+__global__ void __launch_bounds__(RS_THREADS) ransac_debug_five_point_kernel(const float4* __restrict__ samples, int n_samples,
+                                                                             float* __restrict__ E_out, int* __restrict__ count) {
+  const int i = blockIdx.x * RS_THREADS + threadIdx.x;
+  if (i >= n_samples) return;
+  const int idx[5] = {0, 1, 2, 3, 4};
+  float Ec[10][9];
+  const int nc = rs_e5_sample(samples + (int64_t)i * 5, idx, Ec);
+  for (int j = 0; j < 10; ++j)
+    for (int k = 0; k < 9; ++k) E_out[((int64_t)i * 10 + j) * 9 + k] = j < nc ? Ec[j][k] : 0.f;
+  count[i] = nc;
 }
 
 // Test hook: one thread per 7-point sample (7 normalised (x, y, u, v) rows), candidates zero-padded to 3.
@@ -899,8 +1359,8 @@ static int rs_check(const char* what, bool pointers, int n_max, int batch, float
 // hyp -> lo -> final for an epipolar model: one round = one sample per lane, so a block draws RS_THREADS samples per round.
 template <class Model>
 static int rs_launch_epipolar(const char* what, const float* d_p0, const float* d_p1, const int32_t* d_n, const int32_t* d_pair_ids,
-                              int n_max, int batch, float thr, int iters, uint32_t seed, float* d_out, uint8_t* d_inliers,
-                              int32_t* d_n_inliers, void* d_ws, size_t ws_bytes, void* stream) {
+                              RsCams cams, int n_max, int batch, float thr, int iters, uint32_t seed, float* d_out,
+                              uint8_t* d_inliers, int32_t* d_n_inliers, void* d_ws, size_t ws_bytes, void* stream) {
   const int rc = rs_check(what, d_p0 && d_p1 && d_out && d_inliers && d_n_inliers && d_ws, n_max, batch, thr, iters, ws_bytes);
   if (rc != XF_OK) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -909,13 +1369,13 @@ static int rs_launch_epipolar(const char* what, const float* d_p0, const float* 
   const size_t smem = (size_t)n_max * sizeof(float4);
   XF_DYN_SMEM(ransac_hyp_kernel<Model>, smem);
   XF_DYN_SMEM(ransac_lo_kernel<Model>, smem);
-  ransac_hyp_kernel<Model><<<dim3(bpp, batch), RS_THREADS, smem, st>>>(d_p0, d_p1, d_n, d_pair_ids, n_max, thr, rounds, seed,
-                                                                       (RsRecord*)d_ws);
+  ransac_hyp_kernel<Model><<<dim3(bpp, batch), RS_THREADS, smem, st>>>(d_p0, d_p1, d_n, d_pair_ids, cams, n_max, thr, rounds,
+                                                                       seed, (RsRecord*)d_ws);
   XF_LAUNCH_CHECK();
-  ransac_lo_kernel<Model><<<dim3(bpp, batch), RS_THREADS, smem, st>>>(d_p0, d_p1, d_n, n_max, thr, (RsRecord*)d_ws);
+  ransac_lo_kernel<Model><<<dim3(bpp, batch), RS_THREADS, smem, st>>>(d_p0, d_p1, d_n, cams, n_max, thr, (RsRecord*)d_ws);
   XF_LAUNCH_CHECK();
-  ransac_final_kernel<Model><<<batch, RS_THREADS, 0, st>>>(d_p0, d_p1, d_n, n_max, thr, (const RsRecord*)d_ws, bpp, d_out,
-                                                           d_inliers, d_n_inliers);
+  ransac_final_kernel<Model><<<batch, RS_THREADS, 0, st>>>(d_p0, d_p1, d_n, cams, n_max, thr, (const RsRecord*)d_ws, bpp,
+                                                           d_out, d_inliers, d_n_inliers);
   XF_LAUNCH_CHECK();
   return XF_OK;
 }
@@ -951,16 +1411,42 @@ extern "C" int xfeat_ransac_homography(const float* d_pts0, const float* d_pts1,
 extern "C" int xfeat_ransac_essential(const float* d_x0, const float* d_x1, const int32_t* d_n, int n_max, int batch, float thr,
                                       int iters, uint32_t seed, float* d_E, uint8_t* d_inliers, int32_t* d_n_inliers, void* d_ws,
                                       size_t ws_bytes, void* stream) {
-  return xf::rs_launch_epipolar<xf::RsEssential>("ransac_essential", d_x0, d_x1, d_n, nullptr, n_max, batch, thr, iters, seed, d_E,
-                                                 d_inliers, d_n_inliers, d_ws, ws_bytes, stream);
+  return xf::rs_launch_epipolar<xf::RsEssential>("ransac_essential", d_x0, d_x1, d_n, nullptr, xf::RsCams{nullptr, nullptr}, n_max,
+                                                 batch, thr, iters, seed, d_E, d_inliers, d_n_inliers, d_ws, ws_bytes, stream);
 }
 
 extern "C" int xfeat_ransac_fundamental(const float* d_pts0, const float* d_pts1, const int32_t* d_n, const int32_t* d_pair_ids,
                                         int n_max, int batch, float thr_px, int iters, uint32_t seed, float* d_F,
                                         uint8_t* d_inliers, int32_t* d_n_inliers, void* d_ws, size_t ws_bytes, void* stream) {
   // the records hold pixel F after the lo launch: the final launch classifies with `Sampson < thr_px` in pixels
-  return xf::rs_launch_epipolar<xf::RsFundamental>("ransac_fundamental", d_pts0, d_pts1, d_n, d_pair_ids, n_max, batch, thr_px,
-                                                   iters, seed, d_F, d_inliers, d_n_inliers, d_ws, ws_bytes, stream);
+  return xf::rs_launch_epipolar<xf::RsFundamental>("ransac_fundamental", d_pts0, d_pts1, d_n, d_pair_ids, xf::RsCams{nullptr, nullptr},
+                                                   n_max, batch, thr_px, iters, seed, d_F, d_inliers, d_n_inliers, d_ws, ws_bytes,
+                                                   stream);
+}
+
+extern "C" int xfeat_relative_pose(const float* d_pts0, const float* d_pts1, const int32_t* d_n, const float* d_K0,
+                                   const float* d_K1, const int32_t* d_pair_ids, int n_max, int batch, float thr_px, int iters,
+                                   uint32_t seed, float* d_E, float* d_R, float* d_t, uint8_t* d_inliers, int32_t* d_n_inliers,
+                                   int32_t* d_n_front, void* d_ws, size_t ws_bytes, void* stream) {
+  XF_REQUIRE(d_K0 && d_K1 && d_R && d_t && d_n_front, "relative_pose: null pointer");
+  const xf::RsCams cams{d_K0, d_K1};
+  const int rc = xf::rs_launch_epipolar<xf::RsEssential5>("relative_pose", d_pts0, d_pts1, d_n, d_pair_ids, cams, n_max, batch,
+                                                          thr_px, iters, seed, d_E, d_inliers, d_n_inliers, d_ws, ws_bytes,
+                                                          stream);
+  if (rc != XF_OK) return rc;
+  xf::ransac_pose_kernel<<<batch, xf::RS_THREADS, 0, (cudaStream_t)stream>>>(d_pts0, d_pts1, d_n, cams, n_max, d_E, d_inliers,
+                                                                              d_n_inliers, d_R, d_t, d_n_front);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
+}
+
+extern "C" int xfeat_debug_five_point(const float* d_samples, int n_samples, float* d_E, int32_t* d_count, void* stream) {
+  XF_REQUIRE(d_samples && d_E && d_count, "debug_five_point: null pointer");
+  XF_REQUIRE(n_samples > 0 && ((uintptr_t)d_samples & 15) == 0, "debug_five_point: bad arguments (16-byte aligned samples)");
+  xf::ransac_debug_five_point_kernel<<<xf::cdiv(n_samples, xf::RS_THREADS), xf::RS_THREADS, 0, (cudaStream_t)stream>>>(
+      (const float4*)d_samples, n_samples, d_E, d_count);
+  XF_LAUNCH_CHECK();
+  return XF_OK;
 }
 
 extern "C" int xfeat_debug_seven_point(const float* d_samples, int n_samples, float* d_F, int32_t* d_count, void* stream) {

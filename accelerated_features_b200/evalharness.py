@@ -113,21 +113,52 @@ def estimate_pose_gpu(kpts0, kpts1, K0, K1, thresh, iters: int = 8192, seed: int
     return R, t, m
 
 
+def estimate_poses_gpu(kpts0: Sequence[np.ndarray], kpts1: Sequence[np.ndarray], K0: Sequence[np.ndarray],
+                       K1: Sequence[np.ndarray], thresh, iters: int = 1024, seed: int = 0) -> List:
+    """estimate_pose_opencv over a chunk of pairs in ONE batched call of geometry.estimate_relative_pose_batch (five-point
+    RANSAC + cheirality on the GPU, per-pair intrinsics): lists of (N_i,2) pixel keypoints and (3,3) intrinsics -> per pair
+    (R, t, mask) or None, as estimate_pose_opencv returns.  Every pair is seeded as pair 0, so pair i's result is what
+    geometry.estimate_relative_pose(kpts0[i], kpts1[i], K0[i], K1[i], thresh, iters, seed) returns.  At most 8192 keypoints
+    per pair."""
+    import torch
+    from .geometry import estimate_relative_pose_batch
+    B = len(kpts0)
+    if B == 0:
+        return []
+    n = np.array([len(k) for k in kpts0], np.int32)
+    p0 = np.zeros((B, max(int(n.max()), 1), 2), np.float32)
+    p1 = np.zeros_like(p0)
+    for b in range(B):
+        p0[b, :n[b]], p1[b, :n[b]] = kpts0[b], kpts1[b]
+    dev = torch.device("cuda", torch.cuda.current_device())
+    E, R, t, mask, n_inl, _ = estimate_relative_pose_batch(
+        torch.from_numpy(p0).to(dev), torch.from_numpy(p1).to(dev), np.asarray(K0, np.float32), np.asarray(K1, np.float32),
+        torch.from_numpy(n).to(dev), thresh, iters, seed, pair_ids=np.zeros(B, np.int32))
+    R, t, mask, n_inl = R.double().cpu().numpy(), t.double().cpu().numpy(), mask.cpu().numpy(), n_inl.cpu().numpy()
+    return [(R[b], t[b], mask[b, :n[b]].copy()) if n[b] >= 5 and n_inl[b] >= 5 else None for b in range(B)]
+
+
 def run_pose_benchmark(match_pairs, samples: Iterable[dict], ransac_thr: float = 2.5, batch_size: int = 64,
-                       pose_fn=estimate_pose_opencv) -> dict:
+                       pose_fn=estimate_pose_opencv, pose_batch_fn=None) -> dict:
     """run_pose_benchmark (megadepth1500.py:200-237) over batches.  `samples`: dicts with 'image0', 'image1' (H,W,3) uint8 BGR
     (what tensor2bgr produces there), 'scale0', 'scale1', 'K0', 'K1', 'T_0to1' as numpy arrays.  Returns compute_maa's numbers
-    plus the per-pair records."""
+    plus the per-pair records.  `pose_batch_fn` (e.g. estimate_poses_gpu), when given, is called once per chunk with the lists
+    of the chunk's (kpts0, kpts1, K0, K1) and the threshold, instead of pose_fn once per pair."""
     samples = list(samples)
     records = []
     for o in range(0, len(samples), batch_size):
         chunk = samples[o:o + batch_size]
         matches = match_pairs([(d["image0"], d["image1"]) for d in chunk])
-        for d, (src, dst) in zip(chunk, matches):
-            src = src * np.asarray(d["scale0"], np.float32)          # rescale kpts (megadepth1500.py:230-231)
-            dst = dst * np.asarray(d["scale1"], np.float32)
+        scaled = [(src * np.asarray(d["scale0"], np.float32), dst * np.asarray(d["scale1"], np.float32))   # rescale kpts
+                  for d, (src, dst) in zip(chunk, matches)]                                             # (megadepth1500.py:230-231)
+        Ks = [(np.asarray(d["K0"], np.float64), np.asarray(d["K1"], np.float64)) for d in chunk]
+        if pose_batch_fn is not None:
+            rets = pose_batch_fn([s for s, _ in scaled], [s for _, s in scaled], [k for k, _ in Ks], [k for _, k in Ks],
+                                 ransac_thr)
+        else:
+            rets = [pose_fn(src, dst, k0, k1, ransac_thr) for (src, dst), (k0, k1) in zip(scaled, Ks)]
+        for d, (src, _), ret in zip(chunk, scaled, rets):
             rec = {"R_err": np.inf, "t_err": np.inf, "n_matches": len(src)}
-            ret = pose_fn(src, dst, np.asarray(d["K0"], np.float64), np.asarray(d["K1"], np.float64), ransac_thr)
             if ret is not None:
                 R, t, _ = ret
                 rec["t_err"], rec["R_err"] = relative_pose_error(np.asarray(d["T_0to1"], np.float64), R, t)

@@ -11,7 +11,8 @@ host -> device -> host pipeline over a sequence of batches; SURVEY 8f-1), `match
 `match_xfeat_lighterglue_pairs` (a list of pairs into one set of mixed-size images, each image extracted once),
 `match_xfeat_star_pairs` (the same for semi-dense matching: XFeat* over a list of pairs, each image extracted once per scale),
 `tracker` (one reference tracked through a video stream, each frame's step replayed as one CUDA graph; tracker.py), and
-`match_xfeat_verified_pairs` (match_xfeat_pairs followed on the device by a fundamental-matrix RANSAC per pair; geometry.py).
+`match_xfeat_verified_pairs` (match_xfeat_pairs followed on the device by a fundamental-matrix RANSAC per pair; geometry.py),
+and `match_xfeat_pose_pairs` (the same with per-image intrinsics: a five-point relative-pose RANSAC + cheirality per pair).
 """
 from __future__ import annotations
 
@@ -879,12 +880,48 @@ class XFeat(torch.nn.Module):
         plan = PairPlan([pair_image_key(x) for x in images], pairs)
         if len(plan.pairs) == 0:
             return []
-        return self._pairs_matched(images, plan, top_k, min_cossim, "match_xfeat_verified_pairs", (ransac_thr, iters, seed))
+
+        def verify(mk0, mk1, cnt, sel, ids):
+            from .geometry import find_fundamental_batch
+            F, mask, n_inl = find_fundamental_batch(mk0, mk1, cnt, ransac_thr, iters, seed, pair_ids=ids)
+            return {"F": F}, mask, n_inl, {}
+
+        return self._pairs_matched(images, plan, top_k, min_cossim, "match_xfeat_verified_pairs", (verify, 8))
+
+    @torch.inference_mode()
+    def match_xfeat_pose_pairs(self, images, pairs, K, top_k=None, min_cossim=-1, ransac_thr: float = 1.0, iters: int = 1024,
+                               seed: int = 0) -> List[Dict[str, np.ndarray]]:
+        """match_xfeat_pairs (same inputs, same extraction, same matches bit for bit) followed, still on the device, by the
+        calibrated relative pose of geometry.estimate_relative_pose_batch on every pair: the five-point RANSAC + cheirality step
+        (poselib.estimate_relative_pose in the 1500-pair benchmarks) that calibrated pair lists run next.  K: one intrinsic
+        matrix per image, (n_images, 3, 3) or (n_images, 4) as (fx, fy, cx, cy), for the image as fed to this call.
+        Result p: {'mkpts0', 'mkpts1' (N,2), 'inliers' (N,) bool, 'n_inliers' int, 'n_front' int, and 'E', 'R' (3,3), 't' (3,)
+        float64 with X1 = R X0 + t, or None when fewer than 5 inliers support them}.  `ransac_thr` in pixels (threshold
+        ransac_thr / f, f the mean focal length of the pair).  Pair p's samples are seeded by (seed, p), so its result is what
+        estimate_relative_pose_batch gives its matches alone with pair_ids=[p].  One host synchronisation per chunk of pairs.
+        top_k above 8192 is refused."""
+        if top_k is None: top_k = self.top_k
+        if top_k > 8192:
+            raise ValueError(f"match_xfeat_pose_pairs: top_k {top_k} > 8192 (the RANSAC caches at most 8192 matches per pair)")
+        plan = PairPlan([pair_image_key(x) for x in images], pairs)
+        if len(plan.pairs) == 0:
+            return []
+        from .geometry import _intrinsics4, estimate_relative_pose_batch
+        Kimg = _intrinsics4(K, len(images), self.dev)
+
+        def verify(mk0, mk1, cnt, sel, ids):
+            ps = torch.from_numpy(plan.pairs[sel]).to(self.dev)
+            E, R, t, mask, n_inl, n_front = estimate_relative_pose_batch(mk0, mk1, Kimg[ps[:, 0]], Kimg[ps[:, 1]], cnt, ransac_thr,
+                                                                         iters, seed, pair_ids=ids)
+            return {"E": E, "R": R, "t": t}, mask, n_inl, {"n_front": n_front}
+
+        return self._pairs_matched(images, plan, top_k, min_cossim, "match_xfeat_pose_pairs", (verify, 5))
 
     def _pairs_matched(self, images, plan: PairPlan, top_k: int, min_cossim: float, what: str, ransac=None) -> List:
-        """The body of match_xfeat_pairs over a non-empty plan, and with `ransac` = (thr, iters, seed) that of
-        match_xfeat_verified_pairs: each chunk's matches go through find_fundamental_batch on the device before the chunk's one
-        host sync."""
+        """The body of match_xfeat_pairs over a non-empty plan, and with `ransac` = (verify, min_inliers) that of
+        match_xfeat_verified_pairs / match_xfeat_pose_pairs: each chunk's matches go through verify(mk0, mk1, cnt, sel, pair_ids)
+        -> (models, mask, n_inliers, counts), dicts of device tensors, on the device before the chunk's one host sync.  Pair p's
+        record holds each model as float64 (None below min_inliers inliers) and each count as an int."""
         presplit = self._lib.xfeat_get_mnn_impl() in (1, 2, 3)   # else: fp32 descriptors, per-pair gather, xfeat_mnn_match_bounded
         order = plan.match_order()
         tp_all = torch.from_numpy(np.ascontiguousarray(plan.table_pairs[order])).to(self.dev)
@@ -898,9 +935,8 @@ class XFeat(torch.nn.Module):
             mk0, mk1, cnt = self._match_table_pairs(tab, tp, top_k, min_cossim, presplit)
             dev_out = [mk0, mk1, cnt]
             if ransac:
-                from .geometry import find_fundamental_batch
-                F, mask, n_inl = find_fundamental_batch(mk0, mk1, cnt, ransac[0], ransac[1], ransac[2], pair_ids=ids_all[o:o + step])
-                dev_out += [F, mask, n_inl]
+                models, mask, n_inl, counts = ransac[0](mk0, mk1, cnt, sel, ids_all[o:o + step])
+                dev_out += [mask, n_inl, *models.values(), *counts.values()]
             host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in dev_out]
             for h, t in zip(host, dev_out):
                 h.copy_(t, non_blocking=True)
@@ -912,10 +948,15 @@ class XFeat(torch.nn.Module):
                 for b, p in enumerate(sel.tolist()):
                     out[p] = (a0[b, :c[b]].copy(), a1[b, :c[b]].copy())
                 continue
-            Fh, mh, nh = host[3].numpy(), host[4].numpy(), host[5].tolist()
+            mh, nh = host[3].numpy(), host[4].tolist()
+            mods = dict(zip(models, (h.numpy() for h in host[5:5 + len(models)])))
+            cnts = dict(zip(counts, (h.tolist() for h in host[5 + len(models):])))
             for b, p in enumerate(sel.tolist()):
-                out[p] = {"mkpts0": a0[b, :c[b]].copy(), "mkpts1": a1[b, :c[b]].copy(), "inliers": mh[b, :c[b]].copy(),
-                          "n_inliers": nh[b], "F": Fh[b].astype(np.float64) if nh[b] >= 8 else None}
+                rec = {"mkpts0": a0[b, :c[b]].copy(), "mkpts1": a1[b, :c[b]].copy(), "inliers": mh[b, :c[b]].copy(),
+                       "n_inliers": nh[b]}
+                rec.update({k: v[b] for k, v in cnts.items()})
+                rec.update({k: v[b].astype(np.float64) if nh[b] >= ransac[1] else None for k, v in mods.items()})
+                out[p] = rec
         return out
 
     @torch.inference_mode()

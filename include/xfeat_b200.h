@@ -337,6 +337,29 @@ XF_API int xfeat_ransac_fundamental(const float* d_pts0, const float* d_pts1, co
  * x1^T F x0 = 0, unit Frobenius norm, zero past the count; d_count (n_samples) int32, 0-3 (0: degenerate sample). */
 XF_API int xfeat_debug_seven_point(const float* d_samples, int n_samples, float* d_F, int32_t* d_count, void* stream);
 
+/* replaces: the calibrated relative-pose step of the 1500-pair benchmarks (poselib.estimate_relative_pose + cheirality,
+ * modules/eval/megadepth1500.py:98-113; poselib's non-linear refinement is not done).  d_pts0 / d_pts1 (batch, n_max, 2) PIXEL
+ * coordinates, d_n (batch) counts (NULL: n_max each), d_K0 / d_K1 (batch, 4) each pair's intrinsics as (fx, fy, cx, cy).
+ * Points are normalised by K^-1; `iters` 5-point samples (0-10 candidates each, fp64 solver) are scored with MSAC on the
+ * Sampson distance in normalised coordinates against thr_px / f, f = (fx0 + fy0 + fx1 + fy1) / 4; every block's winner is
+ * locally optimised (Sampson-weighted 8-point refits projected onto the essential manifold) and the best one classifies
+ * (inlier iff Sampson distance < thr_px / f).  Then, per pair, the four (R, t) decompositions of E are tested on the inliers
+ * (triangulated depths > 0 in both cameras) and the one with the most points in front wins (first of (R1, t), (R1, -t),
+ * (R2, t), (R2, -t) on a tie).  Outputs d_E (batch, 9) row-major with x1^T E x0 = 0 in normalised coordinates; d_R (batch, 9)
+ * row-major and d_t (batch, 3) unit, X1 = R X0 + t; d_inliers (batch, n_max) 0/1; d_n_inliers (batch), a negative count
+ * (XF_N_OVERFLOW) passed through; d_n_front (batch) inliers in front of both cameras under (R, t).  Fewer than 5 matches, or no
+ * model: zero E, R = I, t = 0, no inliers, n_front 0.  Samples are drawn from (seed, d_pair_ids[b]) (NULL: b).  n_max <= 8192.
+ * Workspace: xfeat_ransac_workspace_bytes. */
+XF_API int xfeat_relative_pose(const float* d_pts0, const float* d_pts1, const int32_t* d_n, const float* d_K0, const float* d_K1,
+                               const int32_t* d_pair_ids, int n_max, int batch, float thr_px, int iters, uint32_t seed,
+                               float* d_E, float* d_R, float* d_t, uint8_t* d_inliers, int32_t* d_n_inliers, int32_t* d_n_front,
+                               void* d_ws, size_t ws_bytes, void* stream);
+
+/* Test hook: the 5-point step of xfeat_relative_pose alone, one sample per thread.  d_samples (n_samples, 5, 4) fp32 rows
+ * (x, y, u, v) in normalised (K^-1) coordinates, 16-byte aligned.  Outputs d_E (n_samples, 10, 9) row-major candidates with
+ * x1^T E x0 = 0, unit Frobenius norm, zero past the count; d_count (n_samples) int32, 0-10 (0: degenerate sample). */
+XF_API int xfeat_debug_five_point(const float* d_samples, int n_samples, float* d_E, int32_t* d_count, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * LighterGlue matcher (csrc/lighterglue.cu; fp32 CUDA-core kernels), its own handle and weight blob
  * ------------------------------------------------------------------------------------------------------- */
